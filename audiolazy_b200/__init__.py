@@ -1,4 +1,4 @@
-"""audiolazy_b200 -- B200-native implementation of AudioLazy's linear-filter hot path.
+"""audiolazy_b200 -- H100-native implementation of AudioLazy's linear-filter hot path.
 
 Same names as the reference (``from audiolazy import ...``) for everything on the path:
 ``Stream``, ``thub``, ``Poly``, ``ZFilter``, ``z``, ``LinearFilter``, ``CascadeFilter``,
@@ -6,7 +6,7 @@ Same names as the reference (``from audiolazy import ...``) for everything on th
 ``gammatone``, ``gammatone_erb_constants``, ``sHz``, ``almost_eq``; plus the bank object
 the reference lacks (``FilterBank``, ``gammatone_bank``, ``erb_space``).
 
-The per-sample recurrences run in hand-written sm_100a CUDA kernels behind the C ABI of
+The per-sample recurrences run in hand-written sm_90a CUDA kernels behind the C ABI of
 ``include/alz_b200.h``; importing this package does not need a GPU, calling a filter does.
 """
 from .core import StrategyDict

@@ -1,6 +1,6 @@
 """Build the native CUDA library in-tree (``audiolazy_b200/_native/libalz_b200.so``).
 
-``nvcc`` cross-compiles for sm_100a without a GPU; the built ``.so`` is git-ignored
+``nvcc`` cross-compiles for sm_90a (H100) without a GPU; the built ``.so`` is git-ignored
 but travels to the GPU box with the repository snapshot. The translation units
 (``csrc/*.cu``: the C ABI plus one unit of kernel instantiations per cascade length) are
 compiled in parallel into ``_native/obj/`` and linked into ONE shared library.
@@ -19,7 +19,7 @@ OBJ_DIR = os.path.join(NATIVE_DIR, "obj")
 LIB_PATH = os.path.join(NATIVE_DIR, "libalz_b200.so")
 INCLUDE = os.path.join(os.path.dirname(_PKG), "include")
 
-ARCH_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH_FLAGS + [
   "-O3", "-lineinfo", "-std=c++17",
   "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",   # only the extern "C" ABI of include/alz_b200.h is exported
@@ -52,7 +52,7 @@ def find_nvcc():
 
 
 def build_native(force: bool = False, verbose: bool = False) -> str:
-  """Compile ``csrc/*.cu`` for sm_100a (only the units that changed) and link the library."""
+  """Compile ``csrc/*.cu`` for sm_90a (only the units that changed) and link the library."""
   if not force and not is_stale():
     return LIB_PATH
   nvcc = find_nvcc()

@@ -28,16 +28,15 @@
 //   * the state buffer holds WORKING-unit values (the host scales memory=/zero= once
 //     in alz_state_init), so no rounding happens at block boundaries.
 //
-// Cost model (B200, measured): DFMA/DMUL with a uniform-register coefficient = 2.06
-// cycles per warp per SM sub-partition, F2F (either direction) ~3.85.  Slaney bank:
-// 12 x 2.06 + 2 x 3.85 = ~32.4 cycles per warp-sample (MONIC mode 2; 34.5 in mode 1): the
-// kernel is FP64-issue bound below the HBM roofline, by construction of the arithmetic the
-// parity bar demands (DESIGN.md section 3).
+// Cost model: a float64-tier warp-sample of the slaney bank issues 12 DFMA/DMUL (uniform-
+// register coefficient) and 2 F2F conversions (MONIC mode 2; mode 1 costs more): the kernel
+// is FP64-issue bound below the HBM roofline, by construction of the arithmetic the parity
+// bar demands (DESIGN.md section 3).
 #pragma once
 #include "alz_lane.cuh"
 
 #ifndef ALZ_GROUP_UNROLL
-#define ALZ_GROUP_UNROLL 8   // groups of 4 samples unrolled in the steady-state loop (8 = the whole tile; measured 2: 4.09, 4: 3.95, 8: 3.92 ms on cfg 4)
+#define ALZ_GROUP_UNROLL 8   // groups of 4 samples unrolled in the steady-state loop (8 = the whole tile)
 #endif
 constexpr int kAlzGroupUnroll = ALZ_GROUP_UNROLL;
 
@@ -222,8 +221,6 @@ struct AlzBiquadCore {
   }
 
   // float32 sample -> float64 section input (with the input-side gain when MONIC == 2)
-  // (Widening normal numbers with integer instructions instead of F2F.F64.F32 -- exponent re-bias +
-  // mantissa shift, conversion unit only for zero/denormal/inf/NaN -- was measured SLOWER: 4.31 vs 3.92 ms.)
   __host__ __device__ __forceinline__ W widen(float x) const { return MONIC == 2 ? (W)(x * Gf) : (W)x; }
 
   // Filter my row of the tile in place: float32 in, float32 out.  `swz` is the XOR

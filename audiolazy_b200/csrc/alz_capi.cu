@@ -290,7 +290,7 @@ int32_t alz_plan_create_ex(const double* coef, const int32_t* desc, int32_t C, i
   p->parallel_sum = (flags & ALZ_PLAN_PARALLEL) != 0;
   if (design_only || cudaDeviceGetAttribute(&p->sm_count, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || p->sm_count <= 0) {
     cudaGetLastError();
-    p->sm_count = 148;
+    p->sm_count = 132;
   }
 
   p->fr_desc.assign((size_t)C * Kmax * 3, 0);
@@ -832,13 +832,13 @@ static bool chunk_geometry(const alz_plan* p, const float* x, const float* y, lo
   const long long slots = (long long)p->sm_count * 24;
   const long long warps = (long long)p->C * ((S + 31) / 32);
   if (warps * 2 > slots) return false;             // the plain launch already fills half of the machine
-  // cost model (measured on B200, tools/time_small.py): a lone warp advances one sample per ~36 ns (12 FP64 ops per
-  // channel-sample); the machine as a whole does ~1.2e12 channel-samples/s and the chunked evaluation runs 2 passes + extras
+  // cost model (tools/time_small.py times both evaluations): a lone warp advances one sample per t_seq / T (12 FP64 ops
+  // per channel-sample); the chunked evaluation runs 2 passes + extras
   const double work = std::max(1, p->fp64_ops) / 12.0;
   const double t_seq = (double)T * 36e-9 * work;
   // Chunk count P (a multiple of 32, chunks of >= 256 samples, <= 1024 because the scan over a stream's chunks is
   // serial): the one with the smallest estimated time.  A pass over all chunks costs ceil(waves) x L samples at the
-  // per-sample time of a warp on a machine `occ` full (36 ns alone ... 92 ns with all 24 warp slots of its SM busy);
+  // per-sample time of a warp on a machine `occ` full (from alone to all 24 warp slots of its SM busy);
   // chunks are whole tiles, so T mod 32 P samples are left over for a sequential tail.
   long long P = 0;
   double best = 1e30;
@@ -847,13 +847,13 @@ static bool chunk_geometry(const alz_plan* p, const float* x, const float* y, lo
     const double occ = waves < 1.0 ? waves : 1.0;
     const long long Lq = T / q / 32 * 32, tail = T - q * Lq;
     const double t_sample = std::max(36e-9, 92e-9 * occ) * work;
-    // + the chunk states: d doubles per (channel, virtual stream), written / scanned / read ~6 times at ~4 TB/s;
+    // + the chunk states: d doubles per (channel, virtual stream), written / scanned / read ~6 times;
     // + ~10 us per wave and pass of CTA start-up and wave-end imbalance; + the serial scan, ~0.1 us per chunk
     const double t_state = 6.0 * p->state_doubles * 8.0 * p->C * (double)S * (double)q / 4e12;
     const double t = 2.0 * std::ceil(waves) * ((double)Lq * t_sample + 1e-5) + t_state + (double)tail * 36e-9 * work + (double)q * 1e-7;
     if (t < best) { best = t; P = q; }
   }
-  if (P == 0 || 1.25 * best + 5e-5 > 0.8 * t_seq) return false;   // the estimate is ~20 % optimistic (measured)
+  if (P == 0 || 1.25 * best + 5e-5 > 0.8 * t_seq) return false;   // the estimate is optimistic
   const long long L = T / P / 32 * 32;
   if (L < 256) return false;
   *P_out = P;
@@ -1323,8 +1323,7 @@ int32_t alz_freq_response_f64(alz_plan* p, const double* w, double* out, int64_t
 
 // ---- pinned host buffers on the GPU's NUMA node ------------------------------------------------
 // alz_apply_f32_host moves 260 B per input sample over PCIe; on a two-socket box a pinned buffer that
-// lives on the other socket halves that rate once several GPUs copy at the same time (round 1: 57.8 ->
-// 39.1 GB/s per GPU at 8 GPUs).  No libnuma in the image: the node comes from sysfs, the policy is set
+// lives on the other socket lowers that rate once several GPUs copy at the same time.  No libnuma in the image: the node comes from sysfs, the policy is set
 // with the mbind system call, the pages are touched here and then registered with CUDA.
 static int gpu_numa_node(int device) {
   char bus[32] = {0};
@@ -1402,7 +1401,7 @@ int32_t alz_host_free(void* ptr) {
 // ---- a stream confined to a partition of the SMs (green context) ----------------------------------------
 // Channel-sharded multi-GPU: every rank's bank kernel is short and its one-warp CTAs sit on ALL SMs for the whole
 // kernel; an NCCL kernel (hundreds of threads x ~100 registers per CTA) needs an SM that is nearly EMPTY, so a broadcast
-// issued on a side stream waits for the bank kernel to end (measured: step = kernel + broadcast).  A stream of a green
+// issued on a side stream waits for the bank kernel to end (a step then costs kernel + broadcast).  A stream of a green
 // context that owns only `sm_count` SMs keeps the bank kernel off the others, which NCCL's CTAs then find free.
 int32_t alz_stream_create_partition(int32_t device, int32_t sm_count, void** stream_out, int32_t* sm_granted) {
   if (!stream_out || sm_count < 8) return fail(ALZ_ERR_INVALID, "bad argument");

@@ -1,4 +1,4 @@
-// alz_lane_tma.cuh -- the "lane = stream" engine with TMA tile movement (sm_100a).
+// alz_lane_tma.cuh -- the "lane = stream" engine with TMA tile movement (sm_90a).
 //
 // Same decomposition as alz_lane.cuh (CTA = warp = (channel, 32 streams), tiles of 32
 // samples filtered in place), but the tile is moved by the Tensor Memory Accelerator:

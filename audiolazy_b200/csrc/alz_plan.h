@@ -46,7 +46,7 @@ struct AlzHostPipe {   // lazily created resources of alz_apply_f32_host
 };
 
 struct alz_plan {
-  int kind = 0, C = 0, K = 0, NB = 0, NB0 = 0, monic = 0, device = 0, sm_count = 148;
+  int kind = 0, C = 0, K = 0, NB = 0, NB0 = 0, monic = 0, device = 0, sm_count = 132;
   int zmask = 0;               // biquad: numerator taps that are zero in every channel (AlzBiquadCore ZMASK)
   int xd = 0, yd = 0;          // history depths exposed to alz_state_init
   int state_doubles = 0;       // per recurrence

@@ -15,7 +15,7 @@ What differs from the reference, by design:
 
 * the per-sample difference equation is not interpreted in Python: a filter call
   flattens the filter into a table of direct-form-I sections and streams blocks of
-  samples through hand-written sm_100a CUDA kernels (:mod:`audiolazy_b200._engine`,
+  samples through hand-written sm_90a CUDA kernels (:mod:`audiolazy_b200._engine`,
   C ABI in ``include/alz_b200.h``). There is no CPU evaluator here: without the
   native library / a CUDA device the call raises.
 * samples cross the device boundary as float32 (the north-star contract); the

@@ -1,5 +1,5 @@
 """Multi-GPU sharding of a filterbank: one process per GPU, ``torch.distributed`` (NCCL
-over NVLink on the B200 box, gloo in CPU tests) for the plumbing.
+over NVLink between H100s, gloo in CPU tests) for the plumbing.
 
 Every (stream, channel) pair is an independent recurrence, so the path shards with no
 data-path collective in steady state (SURVEY.md section 8e):
@@ -223,7 +223,7 @@ class BroadcastPipeline(object):
     self.side = torch.cuda.Stream(device=dev, priority=-1)
     # ``compute_sms``: run the bank kernels on a green-context stream that owns only that many SMs. The kernel's
     # one-warp CTAs otherwise sit on EVERY SM for the whole kernel and an NCCL CTA (hundreds of threads x ~100
-    # registers) needs a nearly empty SM: the side-stream broadcast then waits for the kernel to end (measured).
+    # registers) needs a nearly empty SM: the side-stream broadcast then waits for the kernel to end.
     self.partition = None
     self.compute = None
     if compute_sms == "auto":

@@ -2,7 +2,7 @@
 """Benchmark of the hot path: input samples/s through the 64-channel gammatone ERB bank.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--strategy slaney]
-                  [--sharding streams|channels] [--distribute]
+                  [--sharding streams|channels] [--distribute] [--dump-outputs DIR]
 
 * A STEP is one pass of the bank over one resident batch of synthetic float32 streams:
   per GPU 4096 streams x 16384 samples (BASELINE.json config 4: "64-channel gammatone ERB
@@ -23,9 +23,14 @@
   timed separately against the NVLink rate. ``--distribute`` (stream sharding): the batch starts
   on rank 0 and is scattered inside the timed region.
 * ``cpu_baseline`` (rank 0, N = 1) and ``--impl reference``: the CPU restatement of the
-  reference's evaluator (oracle/, kind "port": the reference itself is pure Python and lives
-  only in the build container) on the host threads this process may use, median of >= 5
+  reference's evaluator (oracle/, kind "port": the reference itself is pure Python and is not
+  part of this repository) on the host threads this process may use, median of >= 5
   repetitions on ONE bounded sample of the same workload.
+* ``--dump-outputs DIR`` (stream sharding): after the K timed steps, rank 0 writes what the last
+  of them returned to its caller -- the outputs of a fixed, seeded sample of 8 streams
+  (``DIR/y.npy``, float32 [8][C][T]) and the carried filter state (``DIR/state.npy``, float64,
+  a seeded sample of it when it exceeds 32 MB). The inputs depend only on the arguments, so
+  two builds can be compared output for output.
 """
 import argparse
 import json
@@ -42,7 +47,8 @@ METRIC = "samples/sec through 64-ch gammatone bank"
 UNIT = "input-samples/s"
 S_PER_GPU, T, C, RATE = 4096, 16384, 64, 48000
 BYTES_PER_IN_SAMPLE = 4 + 4 * C     # SURVEY.md section 8(d)
-NVLINK_GBS = 900.0                  # one direction of NVLink 5 per GPU (B200_PROFILING.md)
+NVLINK_GBS = 450.0                  # one direction of NVLink 4 per H100 SXM (data sheet: 900 GB/s both ways)
+DUMP_STREAMS, DUMP_STATE_BYTES = 8, 32 << 20
 
 
 def parse():
@@ -60,6 +66,7 @@ def parse():
   ap.add_argument("--no-e2e", action="store_true")
   ap.add_argument("--no-cpu", action="store_true")
   ap.add_argument("--no-extras", action="store_true", help="skip the secondary records (strategies, cfg2/3/5, generic, stream API)")
+  ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs (a fixed sample) as DIR/<name>.npy")
   return ap.parse_args()
 
 
@@ -68,16 +75,20 @@ def peaks():
     with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as fh:
       return float(json.load(fh)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, copy read+write)"
   except Exception:
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet HBM3 bandwidth)"
 
 
-def ncu_traffic():
-  """DRAM bytes per launch of the headline kernel from the committed ncu capture."""
-  try:
-    with open(os.path.join(ROOT, "profiles", "ncu_summary.json")) as fh:
-      return json.load(fh).get("dram_bytes_per_launch")
-  except Exception:
-    return None
+def dump_outputs(directory, y, state):
+  """--dump-outputs: the last timed step's y for a seeded sample of streams, and its carried state."""
+  import numpy as np
+  os.makedirs(directory, exist_ok=True)
+  rng = np.random.default_rng(0)
+  streams = np.sort(rng.choice(y.shape[0], min(DUMP_STREAMS, y.shape[0]), replace=False))
+  np.save(os.path.join(directory, "y.npy"), y[streams.tolist()].cpu().numpy())
+  st = state.cpu().numpy()
+  if st.nbytes > DUMP_STATE_BYTES:
+    st = st[np.sort(rng.choice(st.size, DUMP_STATE_BYTES // st.itemsize, replace=False))]
+  np.save(os.path.join(directory, "state.npy"), st)
 
 
 def host_cpus():
@@ -298,7 +309,7 @@ def extras(torch, dev, args, peak):
   import audiolazy_b200 as ab
   from audiolazy_b200 import _capi
   out = {}
-  flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)      # > 126 MB L2
+  flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)      # > 50 MB L2
   S, Tn = args.streams, args.samples
   try:
     strat = {}
@@ -432,6 +443,8 @@ def run_ours(args):
     return float(t.item())
 
   if args.sharding == "channels" and distributed:
+    if args.dump_outputs:
+      raise SystemExit("--dump-outputs: stream sharding only")
     return run_channel_sharded(args, torch, dist, dev, world, rank, local, barrier, max_over_ranks)
 
   S, Tn = args.streams, args.samples
@@ -470,6 +483,8 @@ def run_ours(args):
   launches = _capi.launch_count() - launches0
   clocks = sampler.stop()
   ms_per_step = ms_total / args.steps
+  if args.dump_outputs and rank == 0:
+    dump_outputs(args.dump_outputs, y, state)
   value = world * S * Tn / (ms_per_step * 1e-3)
 
   # ---- sustained: >= sustain_s of back-to-back launches, own clock record --------------------
@@ -547,7 +562,7 @@ def run_ours(args):
     peak, peak_src = peaks()
     achieved = BYTES_PER_IN_SAMPLE * S * Tn / (ms_per_step * 1e-3) / 1e9          # per GPU, GB/s
     roof = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-            "traffic": ncu_traffic(), "peak_source": peak_src,
+            "peak_source": peak_src,
             "burst": {"achieved": achieved, "frac": achieved / peak, "seconds": ms_total * 1e-3},
             "kernel": "alz_biquad_tma_kernel<K=4,NB=2,MONIC=2>: %d of %d channels on the float32 tier (plan-time probe, "
                       "tolerance %.1e), the rest float64; DESIGN.md section 3" % (int(tiers.sum()), len(tiers), plan.tier_tol)}
@@ -565,7 +580,7 @@ def run_ours(args):
                  else "streams (inputs resident per rank, no data-path collective)",
                  "io_dtype": "float32", "arithmetic": "float64 recurrence; float32 recurrence on the channels whose "
                  "plan-time probe error is <= %.1e (%d of %d)" % (plan.tier_tol, int(tiers.sum()), len(tiers)),
-                 "l2": "inputs (%.0f MB) and outputs (%.1f GB) per step exceed the 126 MB L2"
+                 "l2": "inputs (%.0f MB) and outputs (%.1f GB) per step exceed the 50 MB L2"
                  % (S * Tn * 4 / 1e6, S * C * Tn * 4 / 1e9),
                  "realtime_48k_streams": value / RATE},
       "clocks": clocks, "gpu_launches": int(launches),
@@ -762,7 +777,7 @@ def run_channel_sharded(args, torch, dist, dev, world, rank, local, barrier, max
       "config": {"workload": rec["workload"], "sharding": "channels", "streams": S, "samples_per_stream": Tn, "channels": C},
       "clocks": rec["clocks"], "gpu_launches": rec["gpu_launches"],
       "roofline": {"bound": "hbm", "achieved": rec["gbs_per_gpu"], "peak": peak, "unit": "GB/s", "frac": rec["gbs_per_gpu"] / peak,
-                   "traffic": None, "peak_source": peak_src, "note": "per GPU: (4 + 4 x C/N) B per input sample"},
+                   "peak_source": peak_src, "note": "per GPU: (4 + 4 x C/N) B per input sample"},
       "collective": rec["collective"], "nvlink": rec.get("nvlink"), "peer_store": rec.get("peer_store"),
       "e2e": {"value": None, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0,
               "note": "host-buffer figure is reported by the stream-sharded run"},

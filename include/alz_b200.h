@@ -1,5 +1,5 @@
 /*
- * alz_b200.h -- C ABI of the B200-native AudioLazy filter hot path.
+ * alz_b200.h -- C ABI of the H100-native AudioLazy filter hot path.
  *
  * This is the drop-in boundary for ONE path of danilobellini/audiolazy: the
  * sample-by-sample linear filter evaluator and its composites.  The reference

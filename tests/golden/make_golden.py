@@ -1,21 +1,23 @@
 #!/usr/bin/env python
 """Generate the golden fixtures of tests/golden/ by RUNNING THE REFERENCE ITSELF.
 
-Run in the build container (the only place /root/reference exists):
+Run it with a checkout of the reference (danilobellini/audiolazy) at hand:
 
-    python tests/golden/make_golden.py
+    ALZ_REFERENCE=<path of the checkout> python tests/golden/make_golden.py
 
-The reference (danilobellini/audiolazy, pure Python) is imported unmodified from
-/root/reference; nothing of it is copied.  The fixtures pin
-  * the filter *designs* (coefficient lists of every builder on the hot path), and
-  * the *outputs* of the reference's sample-by-sample evaluator on seeded inputs,
-so that oracle/ (and, through it, the CUDA path) can be checked on a box that does
-not have the reference (the GPU box).
+The reference (pure Python) is imported unmodified from that checkout; nothing of it
+is copied.  The fixtures pin
+  * the filter *designs* (coefficient lists of every builder on the hot path),
+  * the *outputs* of the reference's sample-by-sample evaluator on seeded inputs, and
+  * the answers tests/test_reference_live.py and tests/test_callers_io.py compare with
+    (reference_cases.json),
+so that oracle/ (and, through it, the CUDA path) is checked without the reference.
 
 Inputs are float32 samples ``numpy.random.default_rng(seed).uniform(-1, 1, n)`` widened
 to Python floats, exactly as SURVEY.md section 8(d) prescribes; they are regenerated from
 the seed by the tests, not stored.
 """
+import hashlib
 import json
 import os
 import sys
@@ -23,13 +25,14 @@ import warnings
 
 import numpy as np
 
-REF = os.environ.get("ALZ_REFERENCE", "/root/reference")
+REF = os.environ["ALZ_REFERENCE"]
 sys.path.insert(0, REF)
 sys.dont_write_bytecode = True
 warnings.simplefilter("ignore")
 import audiolazy as al  # noqa: E402  (the reference)
 
 HERE = os.path.dirname(os.path.abspath(__file__))
+sys.path.insert(0, os.path.dirname(HERE))
 RATE = 48000
 s, Hz = al.sHz(RATE)
 
@@ -252,6 +255,80 @@ def main():
   np.savez_compressed(os.path.join(HERE, "vectors.npz"), **vectors)
   print("wrote", os.path.join(HERE, "designs.json"), os.path.getsize(os.path.join(HERE, "designs.json")), "bytes")
   print("wrote", os.path.join(HERE, "vectors.npz"), os.path.getsize(os.path.join(HERE, "vectors.npz")), "bytes")
+  reference_cases()
+
+
+def digest(y):
+  """SHA-256 of a float64 array's little-endian bytes: bit-exact equality without storing the array."""
+  return hashlib.sha256(np.ascontiguousarray(y, dtype="<f8").tobytes()).hexdigest()
+
+
+def reference_cases():
+  """reference_cases.json: what the reference answers in tests/test_reference_live.py and
+  tests/test_callers_io.py (long outputs as digests of their float64 bytes)."""
+  import audiolazy_b200 as ab
+  from test_callers_io import make_wav
+  cases = {}
+  # test_oracle_vs_reference_all_64_channels: channels 0, 7, ..., 63 on signal(123, 3000)
+  x = signal(123, 3000)
+  cases["bank_digests"] = {}
+  for name in ("slaney", "klapuri", "sampled"):
+    bank = ab.gammatone_bank(strategy=name)
+    rows = []
+    for c in range(0, 64, 7):
+      fc = bank.freqs[c]
+      bw = al.gammatone_erb_constants(4)[0] * al.erb(fc * Hz, Hz)
+      rows.append(digest(run(al.gammatone[name](fc * Hz, bw), x)))
+    cases["bank_digests"][name] = rows
+  # test_lfilter_grid_like_reference_test: reference tests/test_filters_extdep.py:41-47
+  grid = []
+  for a in [[1.], [3.], [1., 3.], [15., -17.2], [-18., 9.8, 0., 14.3]]:
+    for b in [[1.], [-1.], [1., 0., -1.], [1., 3.]]:
+      for data in [list(range(5)), list(range(5, 0, -1)), [7, 22, -5], [8., 3., 15.]]:
+        grid.append([b, a, data, run(al.ZFilter(b, a), np.asarray(data, dtype=np.float32)).tolist()])
+  cases["lfilter_grid"] = grid
+  # test_random_designs_match_reference_bit_for_bit: the same draws as the test; per draw the digest of the
+  # repr() of its seven filters' [(numlist, denlist), ...] (repr round-trips every float exactly)
+  rng = np.random.default_rng(5)
+  draws = []
+  for _ in range(40):
+    freq, bw, cutoff = rng.uniform(0.01, 3.0), rng.uniform(1e-3, 0.6), rng.uniform(0.01, 3.1)
+    rng.integers(1, 50), rng.integers(1, 50)
+    filts = [al.gammatone.slaney(freq, bw), al.gammatone.klapuri(freq, bw), al.gammatone.sampled(freq, bw),
+             al.gammatone.sampled(freq, bw, phase=0.4, eta=5), al.lowpass.z(cutoff), al.highpass.pole(cutoff),
+             al.resonator.z_exp(freq, bw)]
+    draws.append(hashlib.sha256(repr([sections_of(f) for f in filts]).encode()).hexdigest())
+  cases["random_designs"] = draws
+  # test_memory_semantics_vs_reference
+  xm = signal(9, 50)
+  b, a = [0.3, 0.2, -0.4], [1.5, -0.2, 0.1, 0.05]
+  cases["memory_semantics"] = [[memory, zero, run(al.ZFilter(b, a), xm, memory=memory, zero=zero).tolist()]
+                               for memory, zero in [([0.1, 0.2, 0.3], 0.0), ([0.1], 0.25), ([0.1, 0.2, 0.3, 0.4, 0.5], -1.0),
+                                                    (None, 0.5)]]
+  # test_callers_io: WavStream, chunks, maverage / comb designs
+  values = [0, 100, -100, 32767, -32768, 12345]
+  cases["wavstream_16"] = list(al.WavStream(make_wav(16, 1, values)))
+  wav = {}
+  for bits in (8, 16, 24, 32):
+    top = 1 << (bits - 1)
+    vals = [0, 1, -1, top - 1, -top, top // 3, -(top // 7), 12345 % top, -(54321 % top)]
+    for channels in (1, 2):
+      v = vals if channels == 1 else vals + vals[::-1]
+      wav["%d_%d" % (bits, channels)] = [list(al.WavStream(make_wav(bits, channels, v))),
+                                         list(al.WavStream(make_wav(bits, channels, v), keep=True))]
+  cases["wavstream_every_width"] = wav
+  data = [0.5, -0.25, 1.0, 0.125, -1.0]
+  cases["chunks"] = [[c.hex() for c in al.chunks(data, size=4)],
+                     [c.hex() for c in al.chunks(data, size=2, dfmt="d", padval=9.)]]
+  cases["maverage"] = {"%s_%d" % (name, size): [list(map(float, al.maverage[name](size).numlist)),
+                                                list(map(float, al.maverage[name](size).denlist))]
+                       for size in (1, 3, 8) for name in ("recursive", "fir")}
+  kr = al.comb.tau(2 * np.pi / 0.05, 2e4).linearize()
+  cases["comb_tau_linearized"] = [list(map(float, kr.numlist)), list(map(float, kr.denlist))]
+  path = os.path.join(HERE, "reference_cases.json")
+  with open(path, "w") as fh:
+    json.dump(cases, fh, indent=0)
+  print("wrote", path, os.path.getsize(path), "bytes")
 
 
 if __name__ == "__main__":

@@ -1,6 +1,6 @@
 """bench.py's reference arm runs anywhere (it times the CPU port): its JSON line carries the
-contract's keys.  The GPU arm prints the same keys plus roofline / clocks (checked on the GPU box
-by the driver; profiles/r01_bench_n1.json is a committed sample)."""
+contract's keys.  The GPU arm prints the same keys plus roofline / clocks (profiles/h100_bench_n1.json
+is a committed sample)."""
 import json
 import os
 import subprocess
@@ -24,7 +24,7 @@ def test_reference_arm_line():
 
 
 def test_round2_gpu_sample_has_the_contract_keys_and_the_new_records():
-  line = json.load(open(os.path.join(ROOT, "profiles", "r02_bench_n1.json")))
+  line = json.load(open(os.path.join(ROOT, "profiles", "h100_bench_n1.json")))
   assert KEYS | {"clocks", "gpu_launches", "roofline"} <= set(line)
   roof = line["roofline"]
   assert roof["bound"] == "hbm" and abs(roof["frac"] - roof["achieved"] / roof["peak"]) < 1e-9
@@ -42,7 +42,7 @@ def test_round2_gpu_sample_has_the_contract_keys_and_the_new_records():
 
 
 def test_committed_gpu_sample_has_the_contract_keys():
-  line = json.load(open(os.path.join(ROOT, "profiles", "r01_bench_n1.json")))
+  line = json.load(open(os.path.join(ROOT, "profiles", "h100_bench_n1.json")))
   assert KEYS | {"clocks", "gpu_launches", "roofline"} <= set(line)
   roof = line["roofline"]
   assert roof["bound"] == "hbm" and abs(roof["frac"] - roof["achieved"] / roof["peak"]) < 1e-9

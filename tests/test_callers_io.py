@@ -1,6 +1,9 @@
 """Callers and data formats either side of the path (SURVEY.md 8f): host-side behaviour on CPU,
-against the live reference where it exists; the filtering itself is covered by the gpu tests."""
+against what the reference answers (tests/golden/reference_cases.json); the filtering itself is
+covered by the gpu tests."""
 import io
+import json
+import os
 import struct
 import wave
 
@@ -8,6 +11,13 @@ import numpy as np
 import pytest
 
 import audiolazy_b200 as ab
+from conftest import GOLDEN
+
+
+@pytest.fixture(scope="module")
+def reference():
+  with open(os.path.join(GOLDEN, "reference_cases.json")) as fh:
+    return json.load(fh)
 
 
 def make_wav(bits, channels, values, rate=8000):
@@ -42,7 +52,7 @@ def test_wavstream_decoding(bits):
 
 def test_wavstream_matches_reference(reference):
   values = [0, 100, -100, 32767, -32768, 12345]
-  want = list(reference.WavStream(make_wav(16, 1, values)))
+  want = reference["wavstream_16"]
   assert list(ab.WavStream(make_wav(16, 1, values))) == pytest.approx(want, rel=1e-7, abs=1e-9)
 
 
@@ -53,8 +63,9 @@ def test_wavstream_matches_reference_every_width(reference, bits):
   values = [0, 1, -1, top - 1, -top, top // 3, -(top // 7), 12345 % top, -(54321 % top)]
   for channels in (1, 2):
     vals = values if channels == 1 else values + values[::-1]
-    assert list(ab.WavStream(make_wav(bits, channels, vals))) == list(reference.WavStream(make_wav(bits, channels, vals)))
-    assert list(ab.WavStream(make_wav(bits, channels, vals), keep=True)) == list(reference.WavStream(make_wav(bits, channels, vals), keep=True))
+    floats, ints = reference["wavstream_every_width"]["%d_%d" % (bits, channels)]
+    assert list(ab.WavStream(make_wav(bits, channels, vals))) == floats
+    assert list(ab.WavStream(make_wav(bits, channels, vals), keep=True)) == ints
 
 
 def test_chunks():
@@ -68,8 +79,9 @@ def test_chunks():
 
 def test_chunks_match_reference(reference):
   data = [0.5, -0.25, 1.0, 0.125, -1.0]
-  assert list(ab.chunks(data, size=4)) == list(reference.chunks(data, size=4))
-  assert list(ab.chunks(data, size=2, dfmt="d", padval=9.)) == list(reference.chunks(data, size=2, dfmt="d", padval=9.))
+  want4, want2 = ([bytes.fromhex(c) for c in blocks] for blocks in reference["chunks"])
+  assert list(ab.chunks(data, size=4)) == want4
+  assert list(ab.chunks(data, size=2, dfmt="d", padval=9.)) == want2
 
 
 def test_wav_batch(tmp_path):
@@ -98,8 +110,9 @@ def test_sources_and_maverage_designs():
 def test_designs_match_reference(reference):
   for size in (1, 3, 8):
     for name in ("recursive", "fir"):
-      mine, theirs = ab.maverage[name](size), reference.maverage[name](size)
-      assert mine.numlist == list(theirs.numlist) and mine.denlist == list(theirs.denlist)
+      mine = ab.maverage[name](size)
+      num, den = reference["maverage"]["%s_%d" % (name, size)]
+      assert mine.numlist == num and mine.denlist == den
   ks = ab.comb.tau(2 * np.pi / 0.05, 2e4).linearize()
-  kr = reference.comb.tau(2 * np.pi / 0.05, 2e4).linearize()
-  assert ks.numlist == list(kr.numlist) and ks.denlist == list(kr.denlist)
+  num, den = reference["comb_tau_linearized"]
+  assert ks.numlist == num and ks.denlist == den

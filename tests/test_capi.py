@@ -38,14 +38,14 @@ def test_exports_every_declared_symbol():
   assert _capi.lib().alz_abi_version() == 2
 
 
-def test_sass_is_sm100a_with_fp64_and_uniform_operands():
+def test_sass_is_sm90a_with_fp64_and_uniform_operands():
   import shutil
   import subprocess
   cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
   if not os.path.exists(cuobjdump):
     pytest.skip("cuobjdump not available")
   out = subprocess.run([cuobjdump, "-lelf", _build.LIB_PATH], capture_output=True, text=True).stdout
-  assert "sm_100a" in out
+  assert "sm_90a" in out
   # stream the SASS and stop as soon as both signatures have been seen
   proc = subprocess.Popen([cuobjdump, "-sass", _build.LIB_PATH], stdout=subprocess.PIPE, text=True)
   seen_ur = seen_cp = seen_tma_ld = seen_tma_st = False

@@ -1,10 +1,10 @@
-// Micro-benchmark: what does the B200 FP64 pipe deliver on the *actual* dependency
+// Micro-benchmark: what does the H100 FP64 pipe deliver on the *actual* dependency
 // structure of a 4-section monic biquad cascade (3 DFMA per section, 12 per sample, all
 // operands distinct registers), as a function of resident warps per SM and of the
 // schedule: plain (section after section, as the compiler sees the reference order)
 // versus skewed (section k works on sample n-k: four independent chains per step)?
 // No memory traffic: isolates the arithmetic pipe from the tile I/O.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o microbench_cascade microbench_cascade.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o microbench_cascade microbench_cascade.cu
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>

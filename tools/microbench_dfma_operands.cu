@@ -1,4 +1,4 @@
-// Micro-benchmark: DFMA issue rate on B200 as a function of WHERE the three operands
+// Micro-benchmark: DFMA issue rate on H100 as a function of WHERE the three operands
 // come from (fresh register pairs, registers shared with the previous instruction,
 // uniform registers).  8 independent chains per thread, 16 warps/SM; event-timed.
 #include <cstdio>

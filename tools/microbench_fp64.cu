@@ -1,8 +1,8 @@
-// Micro-benchmarks that size the recurrence kernel's design on B200 (sm_100a):
+// Micro-benchmarks that size the recurrence kernel's design on H100 (sm_90a):
 //   * DFMA issue rate per SM (ILP x warps sweep) and dependent-chain latency
 //   * F2F.F32.F64 / F2F.F64.F32 conversion rate, alone and mixed with DFMA
 //   * FFMA rate for comparison
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o microbench_fp64 microbench_fp64.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o microbench_fp64 microbench_fp64.cu
 // Prints one line per experiment: name, ops/clk/SM (SM clock measured with clock64).
 #include <cstdio>
 #include <cstdlib>

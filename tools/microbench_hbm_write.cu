@@ -1,4 +1,4 @@
-// Micro-benchmark: what is the B200's achievable HBM bandwidth for a WRITE-dominated
+// Micro-benchmark: what is the H100's achievable HBM bandwidth for a WRITE-dominated
 // stream (the filterbank writes 256 B for every 4 B it reads), as opposed to the
 // read+write copy that MEASURED_PEAKS.json's hbm_gbs is defined on?
 //   fill_seq      : grid-stride 16-byte stores over one contiguous 16 GiB buffer
@@ -8,7 +8,7 @@
 //   copy          : read + write (same bytes each way), for the copy-peak cross-check
 //   read          : pure read (sum reduction)
 // Each variant is timed with CUDA events over several repetitions on >= 8 GiB, far
-// beyond the 126 MB L2.
+// beyond the 50 MB L2.
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>

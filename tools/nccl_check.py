@@ -125,10 +125,10 @@ check("state=None is a fresh state every call", torch.equal(ss.apply(x_loc), y_l
 if rank == 0:
   in_bytes, recv = S * T * 4, S * (C - Cl) * T * 4
   print("nccl_check world=%d S=%d T=%d: broadcast %.3f ms (%.0f GB/s); kernel alone %.3f ms, with overlapped broadcast %.3f ms "
-        "(%+.1f %%); in-place all-gather %.3f ms (%.0f GB/s received per GPU = %.2f of 900); fused peer-memory store to rank 0 "
+        "(%+.1f %%); in-place all-gather %.3f ms (%.0f GB/s received per GPU = %.2f of 450); fused peer-memory store to rank 0 "
         "%.3f ms (%.0f GB/s into rank 0); %s" % (
           world, S, T, ms_b, in_bytes / ms_b / 1e6, ms_k, ms_p, 100 * (ms_p / ms_k - 1), ms_g, recv / ms_g / 1e6,
-          recv / ms_g / 1e6 / 900, ms_peer, recv / ms_peer / 1e6 if ms_peer == ms_peer else float("nan"),
+          recv / ms_g / 1e6 / 450, ms_peer, recv / ms_peer / 1e6 if ms_peer == ms_peer else float("nan"),
           "PARITY OK" if not fails else "PARITY FAILED: " + ", ".join(fails)))
 dist.barrier()
 dist.destroy_process_group()

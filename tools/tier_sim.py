@@ -13,8 +13,8 @@ prints each channel's error against the float64 oracle:
   dform2   dform with the numerator taken from the previous section's difference
 
 Round-2 outcome (DESIGN.md section 3): on white noise the difference form holds 1.6e-6 from ERB channel 6 upward
-(direct float32: 1e-3 ... 1e-5 there), but (i) it was built and measured on B200 at 4.0 ms for the arithmetic alone (a
-4-deep dependency chain per section and sample; float64 needs 3.57 ms), (ii) it misses the bar on short rows (64
+(direct float32: 1e-3 ... 1e-5 there), but (i) it needs a 4-deep dependency chain per section and sample for the
+arithmetic alone, (ii) it misses the bar on short rows (64
 samples: 6e-5 relative to the early transient's peak) and on inputs without in-band content (pure Nyquist: 4e-3).
 It is NOT in the product; this script keeps the experiment reproducible.
 
