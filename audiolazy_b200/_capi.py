@@ -168,6 +168,7 @@ class Plan(object):
     self.n_sections = info.n_sections
     self.num_taps = info.num_taps
     self.monic = bool(info.monic)
+    self.monic_mode = info.monic          # 0 plain sections, 1 gain on the float64 output, 2 gain on the float32 input
     self.state_doubles_per_recurrence = info.state_doubles
     self.fp64_ops = info.fp64_ops
     self.device = info.device

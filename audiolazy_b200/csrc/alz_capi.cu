@@ -993,7 +993,9 @@ static int envelope_impl(const alz_plan* p, const float* x, float* env, double* 
                          long long S, long long T, long long xs, long long es, int decim, int mode, double g, double R,
                          cudaStream_t st) {
   AlzTileArgs ta{};
-  ta.x = x; ta.y = env;                      // y only feeds the (unused) output tensor map: any valid 16-byte aligned address
+  // y only feeds the output tensor map, which the envelope consumer never uses; it must be 16-byte aligned for the map to
+  // be encoded, and env need not be (a block of a longer envelope row starts anywhere), so x, which must be, stands in.
+  ta.x = x; ta.y = const_cast<float*>(x);
   ta.S = S; ta.T = T; ta.xs = xs; ta.ys = (T + 3) & ~3LL; ta.ysS = (long long)p->C * ta.ys; ta.C = p->C; ta.Stot = sstride / p->C;
   ta.state = state; ta.sstride = sstride;
   ta.vec_in = (((uintptr_t)x & 15) == 0 && (xs & 3) == 0) ? 1 : 0;

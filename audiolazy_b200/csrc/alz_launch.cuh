@@ -159,11 +159,15 @@ static int launch_biquad_k(const alz_plan* p, const AlzTileArgs& ta, cudaStream_
   }
 }
 
-// head-FIR plans: first section with up to 8 numerator taps (K in {1, 4}, NB in {1, 3})
+// head-FIR plans: first section with up to 8 numerator taps (K in {1, 4}, NB in {1, 3}).  NB counts the taps of the
+// sections AFTER the first, so a one-section plan always has NB = 1: K = 1 is instantiated for NB = 1 only.
 template <int K>
 static int launch_headfir_k(const alz_plan* p, const AlzTileArgs& ta, cudaStream_t st) {
-  if (p->NB <= 1) return launch_biquad_nb<K, 1, 8>(p, ta, st);
-  return launch_biquad_nb<K, 3, 8>(p, ta, st);
+  if constexpr (K == 1) return launch_biquad_nb<1, 1, 8>(p, ta, st);
+  else {
+    if (p->NB <= 1) return launch_biquad_nb<K, 1, 8>(p, ta, st);
+    return launch_biquad_nb<K, 3, 8>(p, ta, st);
+  }
 }
 
 // ---- plan-time tier probe (host) -------------------------------------------------------------
@@ -229,6 +233,9 @@ static double probe_biquad_k(const alz_plan* p, const double* r64, const double*
 
 template <int K>
 static double probe_headfir_k(const alz_plan* p, const double* r64, const double* r32) {
-  if (p->NB <= 1) return probe_biquad_nb<K, 1, 8>(p, r64, r32, p->probe_len);
-  return probe_biquad_nb<K, 3, 8>(p, r64, r32, p->probe_len);
+  if constexpr (K == 1) return probe_biquad_nb<1, 1, 8>(p, r64, r32, p->probe_len);
+  else {
+    if (p->NB <= 1) return probe_biquad_nb<K, 1, 8>(p, r64, r32, p->probe_len);
+    return probe_biquad_nb<K, 3, 8>(p, r64, r32, p->probe_len);
+  }
 }
