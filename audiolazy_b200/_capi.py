@@ -33,6 +33,7 @@ SYMBOLS = (
   "alz_last_error", "alz_abi_version", "alz_device_count", "alz_set_device", "alz_plan_create", "alz_plan_create_ex",
   "alz_plan_destroy", "alz_plan_taps", "alz_apply_tv_f32", "alz_plan_tiers", "alz_apply_f32_ex", "alz_host_alloc",
   "alz_host_free", "alz_stream_create_partition", "alz_stream_destroy_partition", "alz_apply_sum_f32", "alz_apply_envelope_f32", "alz_apply_envelope_f32_host",
+  "alz_apply_envelope_f32_ex", "alz_apply_envelope_f32_host_ex",
   "alz_plan_info_get", "alz_plan_state_doubles", "alz_state_init", "alz_plan_history", "alz_apply_f32",
   "alz_apply_f32_host", "alz_sum_channels_f32", "alz_freq_response_f64", "alz_launch_count",
 )
@@ -103,6 +104,10 @@ def lib():
   L.alz_apply_envelope_f32.argtypes = [vp, vp, vp, vp, vp, i64, i64, i64, i64, i32, i32, f64, f64, vp]
   L.alz_apply_envelope_f32_host.restype = i32
   L.alz_apply_envelope_f32_host.argtypes = [vp, vp, vp, i64, i64, i64, i64, i32, i32, f64, f64]
+  L.alz_apply_envelope_f32_ex.restype = i32
+  L.alz_apply_envelope_f32_ex.argtypes = [vp, vp, vp, vp, vp, i64, i64, i64, i64, i32, i32, i32, f64, f64, vp]
+  L.alz_apply_envelope_f32_host_ex.restype = i32
+  L.alz_apply_envelope_f32_host_ex.argtypes = [vp, vp, vp, vp, vp, i64, i64, i64, i64, i32, i32, i32, f64, f64]
   L.alz_stream_create_partition.restype = i32
   L.alz_stream_create_partition.argtypes = [i32, i32, ctypes.POINTER(vp), ctypes.POINTER(i32)]
   L.alz_stream_destroy_partition.restype = i32
@@ -230,6 +235,37 @@ class Plan(object):
     assert env.dtype == np.float32 and env.shape == (S, self.n_channels, T // decim) and env.flags.c_contiguous
     _check(lib().alz_apply_envelope_f32_host(self._h, x.ctypes.data, env.ctypes.data, S, T, x.strides[0] // 4 if S > 1 else T,
                                              T // decim, int(decim), self.ENVELOPE_MODES[mode], float(g), float(R)))
+    return env
+
+  def apply_envelope_ex(self, x_ptr, env_ptr, state_ptr, env_state_ptr, n_streams, n_samples, x_stride, env_stride, decim,
+                        phase, mode, g, R, stream=0):
+    """:meth:`apply_envelope` for a block of an endless stream (``alz_apply_envelope_f32_ex``): any ``n_samples``;
+    ``phase`` samples of the current decimation window were consumed before the block, which yields
+    ``(phase + n_samples) // decim`` values per row."""
+    _check(lib().alz_apply_envelope_f32_ex(self._h, x_ptr, env_ptr, state_ptr, env_state_ptr, int(n_streams),
+                                           int(n_samples), int(x_stride), int(env_stride), int(decim), int(phase),
+                                           self.ENVELOPE_MODES[mode], float(g), float(R), stream))
+
+  def apply_envelope_host_ex(self, x, env=None, state_ptr=None, env_state_ptr=None, decim=48, phase=0, mode="abs", g=None,
+                             R=None):
+    """:meth:`apply_envelope_host` for a block of an endless stream (``alz_apply_envelope_f32_host_ex``): device states
+    (``None``: zero, discarded) and ``phase``; returns ``env`` [S][C][(phase + T) // decim]."""
+    x = np.asarray(x, dtype=np.float32)
+    if x.ndim == 1:
+      x = x[None, :]
+    if x.strides[1] != 4:
+      x = np.ascontiguousarray(x)
+    S, T = x.shape
+    if g is None or R is None:
+      R = 0.99 if R is None else R
+      g = 1.0 - R if g is None else g
+    n_out = (int(phase) + T) // decim
+    if env is None:
+      env = np.empty((S, self.n_channels, n_out), dtype=np.float32)
+    assert env.dtype == np.float32 and env.shape == (S, self.n_channels, n_out) and env.flags.c_contiguous
+    _check(lib().alz_apply_envelope_f32_host_ex(self._h, x.ctypes.data, env.ctypes.data, state_ptr, env_state_ptr, S, T,
+                                                x.strides[0] // 4 if S > 1 else max(T, 1), max(n_out, 1), int(decim),
+                                                int(phase), self.ENVELOPE_MODES[mode], float(g), float(R)))
     return env
 
   def tiers(self):

@@ -259,9 +259,13 @@ def bank_streams(bank_sections, seq, xinit, yinit):
   """One lazy Stream per channel, fed by a shared pump (like a tee: a channel consumed
   far ahead of the others buffers their samples)."""
   db = device_bank(bank_sections)
-  C = db.n_channels
+  return tee_streams(_pump(db, seq, xinit, yinit, False), db.n_channels)
+
+
+def tee_streams(pump, C):
+  """``pump``: generator of per-block ``[C, n]`` arrays -> ``C`` lazy Streams, one per row, that share it (a row
+  consumed far ahead of the others buffers their blocks)."""
   queues = [deque() for _ in range(C)]
-  pump = _pump(db, seq, xinit, yinit, False)
 
   def channel(c):      # generator of per-block lists of channel c
     while True:

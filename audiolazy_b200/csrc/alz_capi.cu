@@ -823,9 +823,9 @@ static int apply_plain(const alz_plan* p, const float* x, float* y, double* stat
 
 // Time-parallel evaluation pays when the plain launch (one warp per channel and 32 streams, serial in time)
 // would leave most of the machine idle: few streams, long blocks.  P chunks per stream (a multiple of 32, so that
-// a warp's 32 virtual streams are chunks of ONE real stream: 3-D / 4-D tensor maps), L samples each.
-static bool chunk_geometry(const alz_plan* p, const float* x, const float* y, long long S, long long T, long long xs,
-                           long long ys, long long* P_out, long long* L_out) {
+// a warp's 32 virtual streams are chunks of ONE real stream: 3-D / 4-D tensor maps), L samples each.  `passes`: the
+// passes over all chunks the evaluation makes (2 for the bank, 3 for the bank with the envelope consumer).
+static bool chunk_geometry(const alz_plan* p, long long S, long long T, int passes, long long* P_out, long long* L_out) {
   if (p->kind != ALZ_KIND_BIQUAD || p->sequential || env_int("ALZ_NO_TIME_PARALLEL", 0)) return false;
   if (T < std::max(2048, env_int("ALZ_TIME_PARALLEL_MIN", 16384)) || p->state_doubles > 32) return false;
   if (T >= (1ll << 31) || S > 65535) return false;
@@ -833,7 +833,7 @@ static bool chunk_geometry(const alz_plan* p, const float* x, const float* y, lo
   const long long warps = (long long)p->C * ((S + 31) / 32);
   if (warps * 2 > slots) return false;             // the plain launch already fills half of the machine
   // cost model (tools/time_small.py times both evaluations): a lone warp advances one sample per t_seq / T (12 FP64 ops
-  // per channel-sample); the chunked evaluation runs 2 passes + extras
+  // per channel-sample); the chunked evaluation runs `passes` passes + extras
   const double work = std::max(1, p->fp64_ops) / 12.0;
   const double t_seq = (double)T * 36e-9 * work;
   // Chunk count P (a multiple of 32, chunks of >= 256 samples, <= 1024 because the scan over a stream's chunks is
@@ -850,7 +850,7 @@ static bool chunk_geometry(const alz_plan* p, const float* x, const float* y, lo
     // + the chunk states: d doubles per (channel, virtual stream), written / scanned / read ~6 times;
     // + ~10 us per wave and pass of CTA start-up and wave-end imbalance; + the serial scan, ~0.1 us per chunk
     const double t_state = 6.0 * p->state_doubles * 8.0 * p->C * (double)S * (double)q / 4e12;
-    const double t = 2.0 * std::ceil(waves) * ((double)Lq * t_sample + 1e-5) + t_state + (double)tail * 36e-9 * work + (double)q * 1e-7;
+    const double t = passes * std::ceil(waves) * ((double)Lq * t_sample + 1e-5) + t_state + (double)tail * 36e-9 * work + (double)q * 1e-7;
     if (t < best) { best = t; P = q; }
   }
   if (P == 0 || 1.25 * best + 5e-5 > 0.8 * t_seq) return false;   // the estimate is optimistic
@@ -861,19 +861,13 @@ static bool chunk_geometry(const alz_plan* p, const float* x, const float* y, lo
   return true;
 }
 
-static int apply_chunked(const alz_plan* p, const float* x, float* y, double* state, long long sstride, long long S,
-                         long long T, long long xs, long long ys, long long P, long long L, cudaStream_t st) {
+// M = A^L (the chunk transition matrices, d x d per channel) on the device, ordered before the next work on `st`.  It
+// depends on the plan and the chunk length only: computed once per (plan, L), kept in the plan.
+static int chunk_transition(const alz_plan* p, long long L, cudaStream_t st, const double** M_out) {
   const int C = p->C, d = p->state_doubles;
-  const long long Tmain = P * L, V = S * P;        // V virtual streams
-  const size_t nstate = (size_t)d * V * C;
-  keep_async_pool();
-  double *Z1 = nullptr, *Z2 = nullptr, *M = nullptr;
+  double* M = nullptr;
   float *xz = nullptr, *ydum = nullptr;
-  ALZ_CUDA(cudaMallocAsync((void**)&Z1, nstate * 8, st));
-  ALZ_CUDA(cudaMallocAsync((void**)&Z2, nstate * 8, st));
-  ALZ_CUDA(cudaMemsetAsync(Z1, 0, nstate * 8, st));
   int rc = ALZ_OK;
-  // M = A^L depends on the plan and the chunk length only: computed once per (plan, L), kept on the device
   alz_plan* pm = const_cast<alz_plan*>(p);
   cudaEvent_t m_ready = nullptr;
   {
@@ -908,6 +902,22 @@ static int apply_chunked(const alz_plan* p, const float* x, float* y, double* st
     }
     pm->m_cache.push_back({L, M, m_ready});
   }
+  *M_out = M;
+  return rc;
+}
+
+static int apply_chunked(const alz_plan* p, const float* x, float* y, double* state, long long sstride, long long S,
+                         long long T, long long xs, long long ys, long long P, long long L, cudaStream_t st) {
+  const int C = p->C, d = p->state_doubles;
+  const long long Tmain = P * L, V = S * P;        // V virtual streams
+  const size_t nstate = (size_t)d * V * C;
+  keep_async_pool();
+  double *Z1 = nullptr, *Z2 = nullptr;
+  const double* M = nullptr;
+  ALZ_CUDA(cudaMallocAsync((void**)&Z1, nstate * 8, st));
+  ALZ_CUDA(cudaMallocAsync((void**)&Z2, nstate * 8, st));
+  ALZ_CUDA(cudaMemsetAsync(Z1, 0, nstate * 8, st));
+  int rc = chunk_transition(p, L, st, &M);
   AlzTileArgs ta{};
   ta.x = x; ta.y = y; ta.S = V; ta.T = L; ta.xs = xs; ta.ys = ys; ta.ysS = (long long)C * ys; ta.C = C; ta.Stot = V;
   ta.vec_in = (((uintptr_t)x & 15) == 0 && (xs & 3) == 0) ? 1 : 0;          // L is a multiple of 32: chunk starts keep the alignment
@@ -935,7 +945,7 @@ static int apply_impl(const alz_plan* p, const float* x, float* y, double* state
                       long long tv_stride, long long ysS) {
   if (ysS == 0) ysS = (long long)p->C * ys;
   long long P = 0, L = 0;
-  if (!tv && ysS == (long long)p->C * ys && chunk_geometry(p, x, y, S, T, xs, ys, &P, &L))
+  if (!tv && ysS == (long long)p->C * ys && chunk_geometry(p, S, T, 2, &P, &L))
     return apply_chunked(p, x, y, state, sstride, S, T, xs, ys, P, L, st);
   AlzTileArgs ta{};
   ta.T = T; ta.xs = xs; ta.ys = ys; ta.ysS = ysS; ta.C = p->C;
@@ -989,57 +999,160 @@ int32_t alz_apply_f32_ex(const alz_plan* p, const float* x, float* y, double* st
   return rc;
 }
 
+// ---- the bank with the fused envelope consumer ----------------------------------------------------------------------
+// The envelope parameters of one call: the lowpass e[n] = fma(R, e[n-1], g r[n]), decimation and rectifier.
+struct EnvParams { int decim, phase, mode; double g, R; };
+
+static int envelope_launch(const alz_plan* p, const AlzTileArgs& ta, cudaStream_t st) {
+  return p->NB0 == 8 ? alzi_launch_envelope_headfir_k4(p, ta, st) : alzi_launch_envelope_k4(p, ta, st);
+}
+
 static int envelope_impl(const alz_plan* p, const float* x, float* env, double* state, double* env_state, long long sstride,
-                         long long S, long long T, long long xs, long long es, int decim, int mode, double g, double R,
-                         cudaStream_t st) {
+                         long long S, long long T, long long xs, long long es, const EnvParams& ep, cudaStream_t st);
+
+// Time-parallel evaluation of few long streams (the bank's is apply_chunked): every stream is cut into P chunks of L
+// samples (virtual streams), and
+//   pass 1  the bank runs every chunk from a zero state, no output                     -> F_p
+//   scan    alz_chunk_scan_kernel                                                     -> the chunks' true bank states
+//   pass 2  bank from the true states, lowpass from zero, nothing stored               -> Fe_p
+//   scan    alz_chunk_scan_kernel again, on the lowpass: it is linear in its state, so the state after chunk p is
+//           e_{p+1} = Fe_p + R^L e_p, the same affine scan with a one-value state        -> the chunks' true lowpass states
+//   pass 3  bank and lowpass from their true states, values stored at each chunk's decimation phase and offset
+// and the T - P L samples left over continue sequentially.  Exact in exact arithmetic; in float64 the chunk states
+// differ from the sequential ones by rounding only.
+static int envelope_chunked(const alz_plan* p, const float* x, float* env, double* state, double* env_state, long long sstride,
+                            long long S, long long T, long long xs, long long es, const EnvParams& ep, long long P, long long L,
+                            cudaStream_t st) {
+  const int C = p->C, d = p->state_doubles;
+  const long long Tmain = P * L, V = S * P;        // V virtual streams
+  const size_t nstate = (size_t)d * V * C, nenv = (size_t)V * C;
+  keep_async_pool();
+  double *Z1 = nullptr, *Z2 = nullptr, *E = nullptr, *E2 = nullptr, *RL = nullptr;
+  const double* M = nullptr;
+  ALZ_CUDA(cudaMallocAsync((void**)&Z1, nstate * 8, st));
+  ALZ_CUDA(cudaMallocAsync((void**)&Z2, nstate * 8, st));
+  ALZ_CUDA(cudaMallocAsync((void**)&E, nenv * 8, st));
+  ALZ_CUDA(cudaMallocAsync((void**)&E2, nenv * 8, st));
+  ALZ_CUDA(cudaMallocAsync((void**)&RL, (size_t)C * 8, st));
+  ALZ_CUDA(cudaMemsetAsync(Z1, 0, nstate * 8, st));
+  ALZ_CUDA(cudaMemsetAsync(E, 0, nenv * 8, st));
+  {   // the lowpass's chunk transition R^L (float64), one 1 x 1 matrix per channel; pageable source: staged before return
+    const std::vector<double> rl((size_t)C, std::pow(ep.R, (double)L));
+    ALZ_CUDA(cudaMemcpyAsync(RL, rl.data(), (size_t)C * 8, cudaMemcpyHostToDevice, st));
+  }
+  int rc = chunk_transition(p, L, st, &M);
+  AlzTileArgs ta{};
+  // y feeds only the (unused) output tensor map: x stands in, as in the sequential launch
+  ta.x = x; ta.y = const_cast<float*>(x); ta.S = V; ta.T = L; ta.xs = xs; ta.ys = xs; ta.ysS = (long long)C * xs; ta.C = C;
+  ta.Stot = V;
+  ta.vec_in = ta.vec_out = 1;
+  ta.vP = (int)P;
+  if (rc == ALZ_OK) {
+    ta.exp = 2;                                    // pass 1: the plain bank kernel without tile stores
+    rc = apply_launch(p, ta, Z1, V * C, st, nullptr, 0);
+    ta.exp = 0;
+  }
+  if (rc == ALZ_OK) {
+    alz_chunk_scan_kernel<<<dim3((unsigned)C, (unsigned)S), 32, 0, st>>>(Z1, Z2, M, state, sstride, sstride / C, d, C, S, P);
+    ALZ_CUDA(cudaGetLastError());
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    ALZ_CUDA(cudaMemcpyAsync(Z1, Z2, nstate * 8, cudaMemcpyDeviceToDevice, st));   // pass 2 overwrites Z2; pass 3 needs it
+    ta.state = Z2; ta.sstride = V * C;
+    ta.env_out = env; ta.env_es = es; ta.env_state = E; ta.env_g = ep.g; ta.env_R = ep.R; ta.env_decim = ep.decim;
+    ta.env_mode = ep.mode; ta.env_phase = ep.phase;
+    ta.env_store = 0;                              // pass 2: only the final lowpass states
+    rc = envelope_launch(p, ta, st);
+  }
+  if (rc == ALZ_OK) {
+    alz_chunk_scan_kernel<<<dim3((unsigned)C, (unsigned)S), 32, 0, st>>>(E, E2, RL, env_state, nenv, sstride / C, 1, C, S, P);
+    ALZ_CUDA(cudaGetLastError());
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    ta.state = Z1;
+    ta.env_state = E2;
+    ta.env_store = 1;                              // pass 3: the output
+    rc = envelope_launch(p, ta, st);
+  }
+  cudaFreeAsync(Z1, st); cudaFreeAsync(Z2, st); cudaFreeAsync(E, st); cudaFreeAsync(E2, st); cudaFreeAsync(RL, st);
+  if (rc == ALZ_OK && T > Tmain) {                 // left-over samples of all streams: the same decision again
+    EnvParams tail = ep;
+    tail.phase = (int)((ep.phase + Tmain) % ep.decim);
+    rc = envelope_impl(p, x + Tmain, env + (ep.phase + Tmain) / ep.decim, state, env_state, sstride, S, T - Tmain, xs, es, tail, st);
+  }
+  return rc;
+}
+
+// One implementation for every envelope entry.  state: [slot][sstride] bank states; env_state: [C][sstride / C] lowpass
+// states (stream-fastest, like the bank's); env rows [S][C], stride es, (phase + T) / decim values each.  T > 0.
+static int envelope_impl(const alz_plan* p, const float* x, float* env, double* state, double* env_state, long long sstride,
+                         long long S, long long T, long long xs, long long es, const EnvParams& ep, cudaStream_t st) {
+  if (((uintptr_t)x & 15) || (xs & 3) || env_int("ALZ_NO_TMA", 0))
+    return fail(ALZ_ERR_UNSUPPORTED, "envelope consumer needs 16-byte aligned x rows");
+  long long P = 0, L = 0;
+  if (chunk_geometry(p, S, T, 3, &P, &L)) return envelope_chunked(p, x, env, state, env_state, sstride, S, T, xs, es, ep, P, L, st);
   AlzTileArgs ta{};
   // y only feeds the output tensor map, which the envelope consumer never uses; it must be 16-byte aligned for the map to
   // be encoded, and env need not be (a block of a longer envelope row starts anywhere), so x, which must be, stands in.
   ta.x = x; ta.y = const_cast<float*>(x);
   ta.S = S; ta.T = T; ta.xs = xs; ta.ys = (T + 3) & ~3LL; ta.ysS = (long long)p->C * ta.ys; ta.C = p->C; ta.Stot = sstride / p->C;
   ta.state = state; ta.sstride = sstride;
-  ta.vec_in = (((uintptr_t)x & 15) == 0 && (xs & 3) == 0) ? 1 : 0;
+  ta.vec_in = 1;
   ta.vec_out = 1;
-  ta.env_out = env; ta.env_es = es; ta.env_state = env_state; ta.env_g = g; ta.env_R = R; ta.env_decim = decim; ta.env_mode = mode;
-  return p->NB0 == 8 ? alzi_launch_envelope_headfir_k4(p, ta, st) : alzi_launch_envelope_k4(p, ta, st);
+  ta.env_out = env; ta.env_es = es; ta.env_state = env_state; ta.env_g = ep.g; ta.env_R = ep.R; ta.env_decim = ep.decim;
+  ta.env_mode = ep.mode; ta.env_phase = ep.phase; ta.env_store = 1;
+  return envelope_launch(p, ta, st);
 }
 
-static int envelope_check(const alz_plan* p, int64_t S, int64_t T, int64_t xs, int64_t es, int32_t decim, int32_t mode) {
+// whole: the block must hold whole decimation windows (the entries without a phase)
+static int envelope_check(const alz_plan* p, int64_t S, int64_t T, int64_t xs, int64_t es, int32_t decim, int32_t phase,
+                          int32_t mode, bool whole) {
   if (!p) return fail(ALZ_ERR_INVALID, "plan is null");
   if (p->device < 0) return fail(ALZ_ERR_CUDA, "design-only plan: no device");
-  if (S < 0 || T < 0 || decim < 1 || mode < 0 || mode > 2) return fail(ALZ_ERR_INVALID, "bad argument");
-  if (T % decim) return fail(ALZ_ERR_INVALID, "n_samples must be a multiple of the decimation factor");
-  if (xs < T || es < T / decim) return fail(ALZ_ERR_INVALID, "row stride shorter than the row");
+  if (S < 0 || T < 0 || decim < 1 || mode < 0 || mode > 2 || phase < 0 || phase >= decim) return fail(ALZ_ERR_INVALID, "bad argument");
+  if (whole && T % decim) return fail(ALZ_ERR_INVALID, "n_samples must be a multiple of the decimation factor");
+  if (xs < T || es < (phase + T) / decim) return fail(ALZ_ERR_INVALID, "row stride shorter than the row");
   if (p->kind != ALZ_KIND_BIQUAD || p->K != 4 || p->C * ALZ_COEF_STRIDE(4, p->NB0) <= 512 || S > 65535ll * 32)
     return fail(ALZ_ERR_UNSUPPORTED, "the envelope consumer is built for the gammatone banks (4 sections per channel)");
   return ALZ_OK;
 }
 
-int32_t alz_apply_envelope_f32(const alz_plan* p, const float* x, float* env, double* state, double* env_state, int64_t S,
-                               int64_t T, int64_t xs, int64_t es, int32_t decim, int32_t mode, double g, double R,
-                               void* cuda_stream) {
-  const int chk = envelope_check(p, S, T, xs, es, decim, mode);
-  if (chk != ALZ_OK) return chk;
+static int envelope_device(const alz_plan* p, const float* x, float* env, double* state, double* env_state, int64_t S,
+                           int64_t T, int64_t xs, int64_t es, const EnvParams& ep, void* cuda_stream) {
   if (S == 0 || T == 0) return ALZ_OK;
-  if (!x || !env || !state || !env_state) return fail(ALZ_ERR_INVALID, "null buffer");
+  if (!x || !state || !env_state || (!env && (ep.phase + T) / ep.decim > 0)) return fail(ALZ_ERR_INVALID, "null buffer");
   int cur = -1;
   ALZ_CUDA(cudaGetDevice(&cur));
   if (cur != p->device) ALZ_CUDA(cudaSetDevice(p->device));
-  const int rc = envelope_impl(p, x, env, state, env_state, (long long)S * p->C, S, T, xs, es, decim, mode, g, R, (cudaStream_t)cuda_stream);
+  const int rc = envelope_impl(p, x, env, state, env_state, (long long)S * p->C, S, T, xs, es, ep, (cudaStream_t)cuda_stream);
   if (cur != p->device) cudaSetDevice(cur);
   return rc;
 }
 
-int32_t alz_apply_envelope_f32_host(const alz_plan* cp, const float* xh, float* eh, int64_t S, int64_t T, int64_t xs, int64_t es,
-                                    int32_t decim, int32_t mode, double g, double R) {
-  alz_plan* p = const_cast<alz_plan*>(cp);
-  const int chk = envelope_check(p, S, T, xs, es, decim, mode);
+int32_t alz_apply_envelope_f32(const alz_plan* p, const float* x, float* env, double* state, double* env_state, int64_t S,
+                               int64_t T, int64_t xs, int64_t es, int32_t decim, int32_t mode, double g, double R,
+                               void* cuda_stream) {
+  const int chk = envelope_check(p, S, T, xs, es, decim, 0, mode, true);
   if (chk != ALZ_OK) return chk;
+  return envelope_device(p, x, env, state, env_state, S, T, xs, es, EnvParams{decim, 0, mode, g, R}, cuda_stream);
+}
+
+int32_t alz_apply_envelope_f32_ex(const alz_plan* p, const float* x, float* env, double* state, double* env_state, int64_t S,
+                                  int64_t T, int64_t xs, int64_t es, int32_t decim, int32_t phase, int32_t mode, double g,
+                                  double R, void* cuda_stream) {
+  const int chk = envelope_check(p, S, T, xs, es, decim, phase, mode, false);
+  if (chk != ALZ_OK) return chk;
+  return envelope_device(p, x, env, state, env_state, S, T, xs, es, EnvParams{decim, phase, mode, g, R}, cuda_stream);
+}
+
+// Host buffers: chunks of whole streams through the plan's staging pipeline.  state / env_state: device, NULL = zero and
+// discarded (per-chunk staging states when both are NULL).
+static int envelope_host(alz_plan* p, const float* xh, float* eh, double* state, double* env_state, int64_t S, int64_t T,
+                         int64_t xs, int64_t es, const EnvParams& ep) {
   if (S == 0 || T == 0) return ALZ_OK;
-  if (!xh || !eh) return fail(ALZ_ERR_INVALID, "null buffer");
+  if (!xh || (!eh && (ep.phase + T) / ep.decim > 0)) return fail(ALZ_ERR_INVALID, "null buffer");
   std::lock_guard<std::mutex> lock(p->host_mu);
   ALZ_CUDA(cudaSetDevice(p->device));
-  const long long C = p->C, Td = T / decim, Tp = (T + 3) & ~3LL, Tdp = (Td + 3) & ~3LL;
+  const int decim = ep.decim;
+  const long long C = p->C, Td = (ep.phase + T) / decim, Tp = (T + 3) & ~3LL, Tdp = (Td + 3) & ~3LL;
   // chunks of whole streams: <= 64 MiB of input per chunk (the output is decim times smaller than the bank's)
   long long Sc = std::max<long long>(32, (64LL << 20) / (Tp * 4) / 32 * 32);
   if (Sc > S) Sc = S;
@@ -1065,30 +1178,70 @@ int32_t alz_apply_envelope_f32_host(const alz_plan* cp, const float* xh, float* 
     have = need;
     return ALZ_OK;
   };
+  // Given states are indexed for all S streams ([slot][S * C], [C][S]).  When only one of the two is given, the other
+  // gets a zeroed buffer of the same layout for this call.
+  double* own = nullptr;
+  if ((state != nullptr) != (env_state != nullptr)) {
+    const size_t bytes = (size_t)(state ? 1 : p->state_doubles) * S * C * 8;
+    ALZ_CUDA(cudaMalloc((void**)&own, bytes));
+    ALZ_CUDA(cudaMemset(own, 0, bytes));
+    (state ? env_state : state) = own;
+  }
+  const bool given = state != nullptr;
+  // Ordering contract (include/alz_b200.h): given states must be complete, or produced by work on the legacy default
+  // stream: the private pipeline streams are ordered after it.
+  if (given) {
+    ALZ_CUDA(cudaEventRecord(hp.done[0], cudaStreamLegacy));
+    for (int k = 0; k < NB; ++k) ALZ_CUDA(cudaStreamWaitEvent(hp.stream[k], hp.done[0], 0));
+  }
   int rc = grow(hp.dx, hp.dx_bytes, (size_t)Sc * Tp * 4);
   if (rc == ALZ_OK) rc = grow(hp.dy, hp.dy_bytes, (size_t)Sc * C * Tdp * 4);
-  if (rc == ALZ_OK) rc = grow(hp.dst, hp.dst_bytes, (size_t)p->state_doubles * Sc * C * 8);
-  if (rc == ALZ_OK) rc = grow(hp.des, hp.des_bytes, (size_t)Sc * C * 8);
-  if (rc != ALZ_OK) return rc;
+  if (rc == ALZ_OK && !given) rc = grow(hp.dst, hp.dst_bytes, (size_t)p->state_doubles * Sc * C * 8);
+  if (rc == ALZ_OK && !given) rc = grow(hp.des, hp.des_bytes, (size_t)Sc * C * 8);
   int i = 0;
   for (long long s0 = 0; s0 < S && rc == ALZ_OK; s0 += Sc, ++i) {
     const long long n = std::min<long long>(Sc, S - s0);
     const int b = i % NB;
     cudaStream_t st = hp.stream[b];
-    cudaMemsetAsync(hp.dst[b], 0, (size_t)p->state_doubles * n * C * 8, st);
-    cudaMemsetAsync(hp.des[b], 0, (size_t)n * C * 8, st);
+    double* sb = given ? state + s0 : hp.dst[b];
+    double* eb = given ? env_state + s0 : hp.des[b];
+    const long long sstride = given ? S * C : n * C;
+    if (!given) {
+      cudaMemsetAsync(hp.dst[b], 0, (size_t)p->state_doubles * n * C * 8, st);
+      cudaMemsetAsync(hp.des[b], 0, (size_t)n * C * 8, st);
+    }
     cudaError_t e = cudaMemcpy2DAsync(hp.dx[b], Tp * 4, xh + s0 * xs, xs * 4, T * 4, n, cudaMemcpyHostToDevice, st);
     if (e != cudaSuccess) { rc = fail(ALZ_ERR_CUDA, "H2D copy failed: %s", cudaGetErrorString(e)); break; }
-    rc = envelope_impl(p, hp.dx[b], hp.dy[b], hp.dst[b], hp.des[b], n * C, n, T, Tp, Tdp, decim, mode, g, R, st);
+    rc = envelope_impl(p, hp.dx[b], hp.dy[b], sb, eb, sstride, n, T, Tp, Tdp, ep, st);
     if (rc != ALZ_OK) break;
-    e = cudaMemcpy2DAsync(eh + s0 * C * es, es * 4, hp.dy[b], Tdp * 4, Td * 4, n * C, cudaMemcpyDeviceToHost, st);
-    if (e != cudaSuccess) { rc = fail(ALZ_ERR_CUDA, "D2H copy failed: %s", cudaGetErrorString(e)); break; }
+    if (Td > 0) {
+      e = cudaMemcpy2DAsync(eh + s0 * C * es, es * 4, hp.dy[b], Tdp * 4, Td * 4, n * C, cudaMemcpyDeviceToHost, st);
+      if (e != cudaSuccess) { rc = fail(ALZ_ERR_CUDA, "D2H copy failed: %s", cudaGetErrorString(e)); break; }
+    }
   }
   for (int k = 0; k < NB; ++k) {
     cudaError_t e = cudaStreamSynchronize(hp.stream[k]);
     if (e != cudaSuccess && rc == ALZ_OK) rc = fail(ALZ_ERR_CUDA, "pipeline failed: %s", cudaGetErrorString(e));
   }
+  cudaFree(own);
   return rc;
+}
+
+int32_t alz_apply_envelope_f32_host(const alz_plan* cp, const float* xh, float* eh, int64_t S, int64_t T, int64_t xs, int64_t es,
+                                    int32_t decim, int32_t mode, double g, double R) {
+  alz_plan* p = const_cast<alz_plan*>(cp);
+  const int chk = envelope_check(p, S, T, xs, es, decim, 0, mode, true);
+  if (chk != ALZ_OK) return chk;
+  return envelope_host(p, xh, eh, nullptr, nullptr, S, T, xs, es, EnvParams{decim, 0, mode, g, R});
+}
+
+int32_t alz_apply_envelope_f32_host_ex(const alz_plan* cp, const float* xh, float* eh, double* state, double* env_state,
+                                       int64_t S, int64_t T, int64_t xs, int64_t es, int32_t decim, int32_t phase, int32_t mode,
+                                       double g, double R) {
+  alz_plan* p = const_cast<alz_plan*>(cp);
+  const int chk = envelope_check(p, S, T, xs, es, decim, phase, mode, false);
+  if (chk != ALZ_OK) return chk;
+  return envelope_host(p, xh, eh, state, env_state, S, T, xs, es, EnvParams{decim, phase, mode, g, R});
 }
 
 int32_t alz_apply_sum_f32(const alz_plan* p, const float* x, float* out, double* state, int64_t S, int64_t T,

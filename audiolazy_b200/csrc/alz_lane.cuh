@@ -63,11 +63,13 @@ struct AlzTileArgs {
                     // of real stream v / vP; x / y are reached through 3-D / 4-D tensor maps (TMA engine only, vP % 32 == 0)
   // fused envelope consumer (alz_apply_envelope_f32, TMA engine): instead of storing y, every lane follows its channel
   // output with a one-pole lowpass of |y| or y^2 and keeps every env_decim-th value
-  float* env_out;        // [S][C][T / env_decim] rows, stride env_es
+  float* env_out;        // [S][C][(env_phase + T) / env_decim] rows, stride env_es (virtual streams: the REAL stream's row)
   long long env_es;
   double* env_state;     // [C * Stot] lowpass states (in/out)
   double env_g, env_R;   // e[n] = g * r[n] + R * e[n-1]
   int env_decim, env_mode;   // mode 0: r = |y|; 1: r = y^2; 2: r = y^2 and sqrt on output (rms)
+  int env_phase;         // samples of the current decimation window consumed before this block (0 <= env_phase < env_decim)
+  int env_store;         // 0: the envelope values are computed but not stored (only the final lowpass states are wanted)
   int exp;          // ALZ_EXP (profiling experiments, TMA engine; results are garbage): 1 = load only the first
                     // tile group and refilter it, 2 = no tile stores
 };

@@ -78,11 +78,18 @@ struct AlzEnvelopePost {
   float* out;          // next output slot of this lane's (stream, channel) row
   double* st;
   int left;            // samples until the next kept value
-  __device__ __forceinline__ void load(const AlzTileArgs& a, int c, long long s, long long r, long long tbeg) {
+  // Sample t of this launch's row is sample pos = env_phase + tbeg + t of the caller's decimation grid; a value is kept
+  // when pos % env_decim == env_decim - 1, at output index pos / env_decim.  Virtual streams (time-parallel evaluation):
+  // `row` is the real stream and `chunk` the lane's chunk of it (the warp's TMA coordinates): its samples start chunk
+  // chunk lengths (a.T each) into the real stream's grid.  32-bit arithmetic: fewer than 2^31 samples (TMA coordinates).
+  __device__ __forceinline__ void load(const AlzTileArgs& a, int c, long long row, unsigned chunk, long long r, long long tbeg) {
     st = a.env_state + r;
     env = __ldcg(st);
-    out = a.env_out + (s * a.C + c) * a.env_es + tbeg / a.env_decim;
-    left = a.env_decim - (int)(tbeg % a.env_decim);
+    const unsigned pos = (unsigned)a.env_phase + (unsigned)tbeg + chunk * (unsigned)a.T;
+    const unsigned q = pos / (unsigned)a.env_decim;
+    out = a.env_out + (row * a.C + c) * a.env_es + q;
+    // no-store mode: the countdown never reaches zero within a launch (< 2^31 samples), so the tile loop stays as is
+    left = a.env_store ? a.env_decim - (int)(pos - q * (unsigned)a.env_decim) : 0x7fffffff;
   }
   __device__ __forceinline__ void tile(const AlzTileArgs& a, const float* row, int swz, int nvalid, bool valid) {
     for (int j = 0; j < nvalid; ++j) {
@@ -90,7 +97,7 @@ struct AlzEnvelopePost {
       const double r = a.env_mode == 0 ? (double)fabsf(y) : (double)y * (double)y;
       env = fma(a.env_R, env, a.env_g * r);
       if (--left == 0) {
-        if (valid) *out = (float)(a.env_mode == 2 ? sqrt(env) : env);
+        if (valid) *out =(float)(a.env_mode == 2 ? sqrt(env) : env);
         ++out;
         left = a.env_decim;
       }
@@ -153,7 +160,10 @@ __device__ __forceinline__ void alz_run_warp_tma(const AlzTileArgs& a, const Cor
   Core core;
   core.load(a, ca, r, c_local, valid);
   Post post;
-  if constexpr (Post::active) post.load(a, c, valid ? s : a.S - 1, r, tbeg);
+  if constexpr (Post::active) {
+    if (a.vP > 0) post.load(a, c, ld2, (unsigned)(ld1 + lane), r, tbeg);   // lanes past S only feed the unused state
+    else post.load(a, c, valid ? s : a.S - 1, 0u, r, tbeg);
+  }
 
   const int ntiles = (int)((tlen + ALZ_TT - 1) / ALZ_TT);
   const int nfull = (int)(tlen / ALZ_TT);

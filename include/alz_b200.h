@@ -229,8 +229,15 @@ int32_t alz_apply_f32_host(const alz_plan* plan, const float* x_host, float* y_h
  * e[n] = g r[n] + R e[n-1] in float64, and only every decim-th value is stored: env_dev[s][c][n / decim].  The bank's
  * 256 bytes of output per input sample never leave the SM; a host caller receives 256 / decim bytes per input sample.
  * Same values as alz_apply_f32 followed by that lowpass on the float32 y.  For gammatone-bank plans (4 sections per
- * channel); n_samples % decim == 0; x rows 16-byte aligned.  env_state_dev: n_channels * n_streams doubles (in/out),
- * state_dev as alz_apply_f32.  The _host variant takes host buffers (zero initial state), copies inside, synchronous.
+ * channel); n_samples % decim == 0; x rows 16-byte aligned (else ALZ_ERR_UNSUPPORTED).  env_state_dev:
+ * n_channels * n_streams doubles (in/out, index c * n_streams + s), state_dev as alz_apply_f32.  (Exception: a call
+ * whose sequential launch would leave more than half of the GPU idle -- n_channels * ceil(n_streams / 32) warps < half
+ * the resident warp slots -- with n_samples >= 16384 (ALZ_TIME_PARALLEL_MIN) is evaluated time-parallel: every stream is
+ * cut into chunks, all chunks run from a zero state, the chunk transition matrices are scanned, all chunks run again from
+ * their true bank states to give the lowpass's chunk transitions, those are scanned, and all chunks run a third time
+ * from their true bank and lowpass states.  The result agrees with the sequential one to float64 rounding of the chunk
+ * states, ~1e-6 relative at worst.  A plan created with ALZ_PLAN_SEQUENTIAL, or ALZ_NO_TIME_PARALLEL=1, never does this.)
+ * The _host variant takes host buffers (zero initial state), copies inside, synchronous.
  */
 int32_t alz_apply_envelope_f32(const alz_plan* plan, const float* x_dev, float* env_dev, double* state_dev,
                                double* env_state_dev, int64_t n_streams, int64_t n_samples, int64_t x_stride,
@@ -238,6 +245,24 @@ int32_t alz_apply_envelope_f32(const alz_plan* plan, const float* x_dev, float* 
 int32_t alz_apply_envelope_f32_host(const alz_plan* plan, const float* x_host, float* env_host, int64_t n_streams,
                                     int64_t n_samples, int64_t x_stride, int64_t env_stride, int32_t decim, int32_t mode,
                                     double g, double R);
+
+/*
+ * The same for a block of an endless stream: any n_samples >= 0.  `phase` (0 <= phase < decim) is the number of samples
+ * of the current decimation window consumed before this block; the block yields n_out = (phase + n_samples) / decim
+ * values per row, the first of them at block sample decim - 1 - phase, and the next block's phase is
+ * (phase + n_samples) % decim.  env_stride >= n_out.  So a stream cut into blocks of any lengths, with state_dev /
+ * env_state_dev / the phase carried from call to call, gives the same values as one call over the whole stream (bit
+ * for bit when no call is evaluated time-parallel, see above).  alz_apply_envelope_f32 is the phase = 0 case.
+ * The _host variant takes host x / env and DEVICE state_dev / env_state_dev (either may be NULL: zero initial state,
+ * discarded afterwards; ordering as alz_apply_f32_host), synchronous.
+ */
+int32_t alz_apply_envelope_f32_ex(const alz_plan* plan, const float* x_dev, float* env_dev, double* state_dev,
+                                  double* env_state_dev, int64_t n_streams, int64_t n_samples, int64_t x_stride,
+                                  int64_t env_stride, int32_t decim, int32_t phase, int32_t mode, double g, double R,
+                                  void* cuda_stream);
+int32_t alz_apply_envelope_f32_host_ex(const alz_plan* plan, const float* x_host, float* env_host, double* state_dev,
+                                       double* env_state_dev, int64_t n_streams, int64_t n_samples, int64_t x_stride,
+                                       int64_t env_stride, int32_t decim, int32_t phase, int32_t mode, double g, double R);
 
 /*
  * Pinned host buffers for alz_apply_f32_host, placed on the NUMA node of CUDA device `device`
