@@ -1,9 +1,13 @@
-"""Build the native CUDA library in-tree (``audiolazy_b200/_native/libalz_b200.so``).
+"""Build the native CUDA libraries in-tree (``audiolazy_b200/_native/``).
 
-``nvcc`` cross-compiles for sm_90a (H100) without a GPU; the built ``.so`` is git-ignored
-but travels to the GPU box with the repository snapshot. The translation units
-(``csrc/*.cu``: the C ABI plus one unit of kernel instantiations per cascade length) are
-compiled in parallel into ``_native/obj/`` and linked into ONE shared library.
+``nvcc`` cross-compiles for sm_90a (H100) without a GPU; the built ``.so`` files are git-ignored
+but travel to the GPU box with the repository snapshot.
+
+* ``libalz_b200.so``, the filter library: the translation units ``csrc/*.cu`` (the C ABI plus
+  one unit of kernel instantiations per cascade length) are compiled in parallel into
+  ``_native/obj/`` and linked into ONE shared library.
+* ``libalz_b200_amdf.so``, the AMDF library: ``csrc_amdf/*.cu`` behind ``include/alz_b200_amdf.h``,
+  compiled with ``-fmad=false`` (its float64 arithmetic reproduces AudioLazy's bit for bit).
 """
 from __future__ import annotations
 
@@ -18,6 +22,9 @@ NATIVE_DIR = os.path.join(_PKG, "_native")
 OBJ_DIR = os.path.join(NATIVE_DIR, "obj")
 LIB_PATH = os.path.join(NATIVE_DIR, "libalz_b200.so")
 INCLUDE = os.path.join(os.path.dirname(_PKG), "include")
+AMDF_CSRC = os.path.join(_PKG, "csrc_amdf")
+AMDF_LIB_PATH = os.path.join(NATIVE_DIR, "libalz_b200_amdf.so")
+AMDF_HEADER = os.path.join(INCLUDE, "alz_b200_amdf.h")
 
 ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH_FLAGS + [
@@ -52,7 +59,36 @@ def find_nvcc():
 
 
 def build_native(force: bool = False, verbose: bool = False) -> str:
-  """Compile ``csrc/*.cu`` for sm_90a (only the units that changed) and link the library."""
+  """Build both libraries (see :func:`build_filters` and :func:`build_amdf`); returns the filter library's path."""
+  path = build_filters(force=force, verbose=verbose)
+  build_amdf(force=force, verbose=verbose)
+  return path
+
+
+def _amdf_sources():
+  return sorted(os.path.join(AMDF_CSRC, f) for f in os.listdir(AMDF_CSRC) if f.endswith((".cu", ".cuh", ".h"))) + \
+         [AMDF_HEADER]
+
+
+def build_amdf(force: bool = False, verbose: bool = False) -> str:
+  """Compile ``csrc_amdf/*.cu`` for sm_90a with ``-fmad=false`` and link ``libalz_b200_amdf.so``."""
+  if not force and os.path.exists(AMDF_LIB_PATH) and \
+     all(os.path.getmtime(s) <= os.path.getmtime(AMDF_LIB_PATH) for s in _amdf_sources()):
+    return AMDF_LIB_PATH
+  nvcc = find_nvcc()
+  if nvcc is None:
+    raise RuntimeError("nvcc not found: cannot build audiolazy_b200's AMDF library")
+  os.makedirs(NATIVE_DIR, exist_ok=True)
+  units = sorted(os.path.join(AMDF_CSRC, f) for f in os.listdir(AMDF_CSRC) if f.endswith(".cu"))
+  tmp = AMDF_LIB_PATH + ".tmp.%d" % os.getpid()
+  cmd = [nvcc] + NVCC_FLAGS + ["-fmad=false"] + (["-Xptxas", "-v"] if verbose else []) + ["-shared", "-o", tmp] + units
+  subprocess.check_call(cmd)
+  os.replace(tmp, AMDF_LIB_PATH)
+  return AMDF_LIB_PATH
+
+
+def build_filters(force: bool = False, verbose: bool = False) -> str:
+  """Compile ``csrc/*.cu`` for sm_90a (only the units that changed) and link the filter library."""
   if not force and not is_stale():
     return LIB_PATH
   nvcc = find_nvcc()

@@ -1,5 +1,5 @@
 """Small helpers the filter path and its tests use: ``sHz``, ``almost_eq``,
-``zero_pad``, ``elementwise`` (reference ``audiolazy/lazy_misc.py``)."""
+``zero_pad``, ``elementwise``, ``freq2lag`` / ``lag2freq`` (reference ``audiolazy/lazy_misc.py``)."""
 from __future__ import annotations
 
 import functools
@@ -9,7 +9,7 @@ from math import pi
 
 from .core import StrategyDict
 
-__all__ = ["sHz", "almost_eq", "zero_pad", "elementwise", "rint", "DEFAULT_SAMPLE_RATE"]
+__all__ = ["sHz", "almost_eq", "zero_pad", "elementwise", "rint", "freq2lag", "lag2freq", "DEFAULT_SAMPLE_RATE"]
 
 DEFAULT_SAMPLE_RATE = 44100   # reference lazy_misc.py:41
 
@@ -23,6 +23,16 @@ def sHz(rate):
   """``(s, Hz)`` unit constants: samples per second and radians per sample per hertz,
   so that ``440 * Hz`` is a frequency in rad/sample (reference ``lazy_misc.py:300-320``)."""
   return float(rate), 2 * pi / rate
+
+
+def freq2lag(v):
+  """Frequency (rad/sample) to lag (samples): ``2 * pi / v`` (reference ``lazy_misc.py:323-325``)."""
+  return 2 * pi / v
+
+
+def lag2freq(v):
+  """Lag (samples) to frequency (rad/sample): ``2 * pi / v`` (reference ``lazy_misc.py:329-331``)."""
+  return 2 * pi / v
 
 
 def zero_pad(seq, left=0, right=0, zero=0.0):
