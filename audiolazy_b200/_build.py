@@ -8,6 +8,7 @@ but travel to the GPU box with the repository snapshot.
   ``_native/obj/`` and linked into ONE shared library.
 * ``libalz_b200_amdf.so``, the AMDF library: ``csrc_amdf/*.cu`` behind ``include/alz_b200_amdf.h``,
   compiled with ``-fmad=false`` (its float64 arithmetic reproduces AudioLazy's bit for bit).
+* ``libalz_b200_zcross.so``, the zero-crossing library: ``csrc_zcross/*.cu`` behind ``include/alz_b200_zcross.h``.
 """
 from __future__ import annotations
 
@@ -25,6 +26,9 @@ INCLUDE = os.path.join(os.path.dirname(_PKG), "include")
 AMDF_CSRC = os.path.join(_PKG, "csrc_amdf")
 AMDF_LIB_PATH = os.path.join(NATIVE_DIR, "libalz_b200_amdf.so")
 AMDF_HEADER = os.path.join(INCLUDE, "alz_b200_amdf.h")
+ZCROSS_CSRC = os.path.join(_PKG, "csrc_zcross")
+ZCROSS_LIB_PATH = os.path.join(NATIVE_DIR, "libalz_b200_zcross.so")
+ZCROSS_HEADER = os.path.join(INCLUDE, "alz_b200_zcross.h")
 
 ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH_FLAGS + [
@@ -59,9 +63,11 @@ def find_nvcc():
 
 
 def build_native(force: bool = False, verbose: bool = False) -> str:
-  """Build both libraries (see :func:`build_filters` and :func:`build_amdf`); returns the filter library's path."""
+  """Build the three libraries (see :func:`build_filters`, :func:`build_amdf` and :func:`build_zcross`); returns the
+  filter library's path."""
   path = build_filters(force=force, verbose=verbose)
   build_amdf(force=force, verbose=verbose)
+  build_zcross(force=force, verbose=verbose)
   return path
 
 
@@ -85,6 +91,28 @@ def build_amdf(force: bool = False, verbose: bool = False) -> str:
   subprocess.check_call(cmd)
   os.replace(tmp, AMDF_LIB_PATH)
   return AMDF_LIB_PATH
+
+
+def _zcross_sources():
+  return sorted(os.path.join(ZCROSS_CSRC, f) for f in os.listdir(ZCROSS_CSRC) if f.endswith((".cu", ".cuh", ".h"))) + \
+         [ZCROSS_HEADER]
+
+
+def build_zcross(force: bool = False, verbose: bool = False) -> str:
+  """Compile ``csrc_zcross/*.cu`` for sm_90a and link ``libalz_b200_zcross.so``."""
+  if not force and os.path.exists(ZCROSS_LIB_PATH) and \
+     all(os.path.getmtime(s) <= os.path.getmtime(ZCROSS_LIB_PATH) for s in _zcross_sources()):
+    return ZCROSS_LIB_PATH
+  nvcc = find_nvcc()
+  if nvcc is None:
+    raise RuntimeError("nvcc not found: cannot build audiolazy_b200's zero-crossing library")
+  os.makedirs(NATIVE_DIR, exist_ok=True)
+  units = sorted(os.path.join(ZCROSS_CSRC, f) for f in os.listdir(ZCROSS_CSRC) if f.endswith(".cu"))
+  tmp = ZCROSS_LIB_PATH + ".tmp.%d" % os.getpid()
+  cmd = [nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-shared", "-o", tmp] + units
+  subprocess.check_call(cmd)
+  os.replace(tmp, ZCROSS_LIB_PATH)
+  return ZCROSS_LIB_PATH
 
 
 def build_filters(force: bool = False, verbose: bool = False) -> str:
