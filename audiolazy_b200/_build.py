@@ -9,6 +9,8 @@ but travel to the GPU box with the repository snapshot.
 * ``libalz_b200_amdf.so``, the AMDF library: ``csrc_amdf/*.cu`` behind ``include/alz_b200_amdf.h``,
   compiled with ``-fmad=false`` (its float64 arithmetic reproduces AudioLazy's bit for bit).
 * ``libalz_b200_zcross.so``, the zero-crossing library: ``csrc_zcross/*.cu`` behind ``include/alz_b200_zcross.h``.
+* ``libalz_b200_lpc.so``, the frame-wise LPC library: ``csrc_lpc/*.cu`` behind ``include/alz_b200_lpc.h``, compiled
+  with ``-fmad=false`` (its float64 sums reproduce AudioLazy's bit for bit).
 """
 from __future__ import annotations
 
@@ -29,6 +31,9 @@ AMDF_HEADER = os.path.join(INCLUDE, "alz_b200_amdf.h")
 ZCROSS_CSRC = os.path.join(_PKG, "csrc_zcross")
 ZCROSS_LIB_PATH = os.path.join(NATIVE_DIR, "libalz_b200_zcross.so")
 ZCROSS_HEADER = os.path.join(INCLUDE, "alz_b200_zcross.h")
+LPC_CSRC = os.path.join(_PKG, "csrc_lpc")
+LPC_LIB_PATH = os.path.join(NATIVE_DIR, "libalz_b200_lpc.so")
+LPC_HEADER = os.path.join(INCLUDE, "alz_b200_lpc.h")
 
 ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH_FLAGS + [
@@ -63,11 +68,12 @@ def find_nvcc():
 
 
 def build_native(force: bool = False, verbose: bool = False) -> str:
-  """Build the three libraries (see :func:`build_filters`, :func:`build_amdf` and :func:`build_zcross`); returns the
-  filter library's path."""
+  """Build the four libraries (see :func:`build_filters`, :func:`build_amdf`, :func:`build_zcross` and
+  :func:`build_lpc`); returns the filter library's path."""
   path = build_filters(force=force, verbose=verbose)
   build_amdf(force=force, verbose=verbose)
   build_zcross(force=force, verbose=verbose)
+  build_lpc(force=force, verbose=verbose)
   return path
 
 
@@ -113,6 +119,28 @@ def build_zcross(force: bool = False, verbose: bool = False) -> str:
   subprocess.check_call(cmd)
   os.replace(tmp, ZCROSS_LIB_PATH)
   return ZCROSS_LIB_PATH
+
+
+def _lpc_sources():
+  return sorted(os.path.join(LPC_CSRC, f) for f in os.listdir(LPC_CSRC) if f.endswith((".cu", ".cuh", ".h"))) + \
+         [LPC_HEADER]
+
+
+def build_lpc(force: bool = False, verbose: bool = False) -> str:
+  """Compile ``csrc_lpc/*.cu`` for sm_90a with ``-fmad=false`` and link ``libalz_b200_lpc.so``."""
+  if not force and os.path.exists(LPC_LIB_PATH) and \
+     all(os.path.getmtime(s) <= os.path.getmtime(LPC_LIB_PATH) for s in _lpc_sources()):
+    return LPC_LIB_PATH
+  nvcc = find_nvcc()
+  if nvcc is None:
+    raise RuntimeError("nvcc not found: cannot build audiolazy_b200's LPC library")
+  os.makedirs(NATIVE_DIR, exist_ok=True)
+  units = sorted(os.path.join(LPC_CSRC, f) for f in os.listdir(LPC_CSRC) if f.endswith(".cu"))
+  tmp = LPC_LIB_PATH + ".tmp.%d" % os.getpid()
+  cmd = [nvcc] + NVCC_FLAGS + ["-fmad=false"] + (["-Xptxas", "-v"] if verbose else []) + ["-shared", "-o", tmp] + units
+  subprocess.check_call(cmd)
+  os.replace(tmp, LPC_LIB_PATH)
+  return LPC_LIB_PATH
 
 
 def build_filters(force: bool = False, verbose: bool = False) -> str:

@@ -7,17 +7,30 @@ generic ring kernel). Mirrors reference ``audiolazy/lazy_lpc.py`` (strategy name
 attribute, exceptions) and ``acorr`` / ``lag_matrix`` of ``lazy_analysis.py:277-342``; the
 recursions here work on coefficient lists, not on filter algebra, so results agree with the
 reference to rounding (tests: 1e-9 relative), not bit for bit.
+
+Frame-wise analysis runs on the GPU (``include/alz_b200_lpc.h``): :class:`LpcFrames` evaluates
+``lpc.kautocor`` of every block of ``Stream(x).blocks(size, hop)`` of many streams, continued block
+by block through an :class:`LpcState`, and :func:`lpc_frames` is its lazy form.  Those follow the
+reference's arithmetic operation for operation (CPython 3.12's compensated ``sum()`` included), so
+they equal ``lpc.kautocor`` of the reference bit for bit.
 """
 from __future__ import annotations
 
 import cmath
+import collections
+import ctypes
 import itertools as it
+import os
+from numbers import Integral, Real
 
+from . import _build, _capi, _engine
 from .core import StrategyDict
+from .crossing import n_blocks
 from .filters import ZFilter
+from .stream import Stream
 
 __all__ = ["ParCorError", "acorr", "lag_matrix", "toeplitz", "levinson_durbin", "lpc", "parcor",
-           "parcor_stable", "lsf", "lsf_stable"]
+           "parcor_stable", "lsf", "lsf_stable", "LpcFrames", "LpcState", "lpc_frames"]
 
 
 class ParCorError(ZeroDivisionError):
@@ -229,3 +242,225 @@ def lsf_stable(filt):
   """True when the LSFs of the two polynomials strictly alternate (``lazy_lpc.py:460-487``)."""
   data = lsf(ZFilter(filt.denpoly))
   return all(x < y for x, y in zip(data, data[1:]))
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Frame-wise LPC on the GPU (include/alz_b200_lpc.h)
+# ---------------------------------------------------------------------------------------------------------------------
+
+#: every function include/alz_b200_lpc.h declares
+SYMBOLS = ("alz_lpc_last_error", "alz_lpc_frames", "alz_lpc_state_bytes", "alz_lpc_state_init", "alz_lpc_scratch_bytes",
+           "alz_lpc_apply_f32")
+MAX_ORDER = 64
+MAX_SIZE = 8192
+
+_lib = None
+
+
+def lib():
+  """Load (once) ``_native/libalz_b200_lpc.so``; raise :class:`~audiolazy_b200._capi.NativeError` if absent."""
+  global _lib
+  if _lib is not None:
+    return _lib
+  path = _build.LPC_LIB_PATH
+  if not os.path.exists(path):
+    raise _capi.NativeError("audiolazy_b200 LPC library not found at %s -- build it with "
+                            "`python -c 'import __graft_entry__ as g; g.build()'` (there is no CPU fallback)" % path)
+  L = ctypes.CDLL(path)
+  i32, i64, vp = ctypes.c_int32, ctypes.c_int64, ctypes.c_void_p
+  L.alz_lpc_last_error.restype = ctypes.c_char_p
+  L.alz_lpc_last_error.argtypes = []
+  L.alz_lpc_frames.restype = i64
+  L.alz_lpc_frames.argtypes = [i64, i64, i32, i32, i32]
+  L.alz_lpc_state_bytes.restype = i64
+  L.alz_lpc_state_bytes.argtypes = [i64, i32]
+  L.alz_lpc_state_init.restype = i32
+  L.alz_lpc_state_init.argtypes = [vp, i64, i32, vp]
+  L.alz_lpc_scratch_bytes.restype = i64
+  L.alz_lpc_scratch_bytes.argtypes = [i64, i64, i32]
+  L.alz_lpc_apply_f32.restype = i32
+  L.alz_lpc_apply_f32.argtypes = [vp, i64, vp, vp, vp, vp, vp, i64, vp, i64, i64, i32, i32, i32, i32, vp, i64, vp]
+  _lib = L
+  return L
+
+
+def _check(rc):
+  if rc < 0:
+    msg = lib().alz_lpc_last_error().decode("utf-8", "replace")
+    if rc == _capi.ALZ_ERR_INVALID:
+      raise ValueError(msg)
+    raise _capi.NativeError("alz_lpc error %d: %s" % (rc, msg))
+  return rc
+
+
+def _int_arg(name, value, lo, hi):
+  if not isinstance(value, Integral) or isinstance(value, bool):
+    raise TypeError("%s must be an integer, not %s" % (name, type(value).__name__))
+  if not lo <= value <= hi:
+    raise ValueError("%s must be in %d .. %d (got %d)" % (name, lo, hi, value))
+  return int(value)
+
+
+LpcResult = collections.namedtuple("LpcResult", ["coef", "error", "failed"])
+
+
+class LpcState(object):
+  """Device state of :class:`LpcFrames` calls over ``n_streams`` streams: per stream the samples consumed and the last
+  ``size`` samples, which hold what the open frames still need.  It is made for one :class:`LpcFrames` (order, size,
+  hop, window), stream count and device; a call with ``final=True`` ends it."""
+
+  def __init__(self, frames, n_streams):
+    torch = _engine.torch_mod()
+    self.n_streams = int(n_streams)
+    if self.n_streams < 0:
+      raise ValueError("n_streams must be >= 0")
+    self.key = frames._key()
+    self.consumed = 0
+    self.ended = False
+    device = torch.device("cuda", torch.cuda.current_device())
+    with torch.cuda.device(device):
+      nbytes = _check(lib().alz_lpc_state_bytes(self.n_streams, frames.size))
+      self.tensor = torch.empty(max(8, nbytes), dtype=torch.uint8, device=device)
+      _check(lib().alz_lpc_state_init(self.tensor.data_ptr(), self.n_streams, frames.size,
+                                      torch.cuda.current_stream(device).cuda_stream))
+
+  @property
+  def device(self):
+    return self.tensor.device
+
+
+class LpcFrames(object):
+  """Linear prediction (autocorrelation method, Levinson-Durbin) of every frame of many streams: frame ``k`` is the
+  block ``[k hop, k hop + size)`` of ``Stream(x).blocks(size, hop)`` (``hop`` defaults to ``size``), times ``window``
+  when one is given (``size`` reals), and its result equals the reference's ``lpc.kautocor(block, order)`` bit for bit.
+
+  * ``lp.apply(x, state=None, final=False)`` -> :class:`LpcResult` ``(coef [S, F, order + 1] float64, error [S, F]
+    float64, failed [S, F] uint8)`` for a CUDA float32 ``x[S, T]``: the F frames this call completes, plus, with
+    ``final=True``, the reference's padded last block when it emits one.  ``coef[..., 0]`` is 1 and coefficients the
+    reference drops as zero are 0.0; ``failed`` marks the frames where the reference raises :class:`ParCorError`
+    (their coef and error are NaN).
+  * ``lp.acorr(x, state=None, final=False)`` -> the lags ``[S, F, order + 1]`` float64 of the same frames.
+  * ``lp.new_state(S)`` -> :class:`LpcState`, to continue streams block by block; blocks of any lengths give the same
+    bits as one call."""
+
+  def __init__(self, order, size, hop=None, window=None):
+    self.order = _int_arg("order", order, 0, MAX_ORDER)
+    self.size = _int_arg("size", size, 1, MAX_SIZE)
+    self.hop = self.size if hop is None else _int_arg("hop", hop, 1, 2 ** 31 - 1)
+    if window is None:
+      self.window = None
+    else:
+      try:
+        values = list(window)
+      except TypeError:
+        raise TypeError("window must be a sequence of %d reals" % self.size)
+      if not all(isinstance(v, Real) for v in values):
+        raise TypeError("window must be a sequence of reals")
+      if len(values) != self.size:
+        raise ValueError("window has %d values, size is %d" % (len(values), self.size))
+      self.window = tuple(float(v) for v in values)
+    self._windows = {}
+
+  def _key(self):
+    return (self.order, self.size, self.hop, self.window)
+
+  def new_state(self, n_streams):
+    return LpcState(self, n_streams)
+
+  def n_frames(self, consumed, T, final):
+    """Frames a call on ``T`` samples emits after ``consumed`` samples (the block count of ``zcross``'s counts)."""
+    return n_blocks(consumed, T, self.size, self.hop, final)
+
+  def _window(self, device):
+    if self.window is None:
+      return None
+    w = self._windows.get(device)
+    if w is None:
+      torch = _engine.torch_mod()
+      w = self._windows[device] = torch.tensor(self.window, dtype=torch.float64, device=device)
+    return w
+
+  def _check_state(self, state, S, device):
+    if not isinstance(state, LpcState):
+      raise ValueError("state must come from LpcFrames.new_state")
+    if state.key != self._key():
+      raise ValueError("state belongs to an LpcFrames with another order, size, hop or window")
+    if state.n_streams != S:
+      raise ValueError("state was created for %d streams, x has %d" % (state.n_streams, S))
+    if state.device != device:
+      raise ValueError("state lives on %s, x on %s" % (state.device, device))
+    if state.ended:
+      raise ValueError("state was ended by a call with final=True")
+
+  def _run(self, x, state, final, levinson):
+    torch = _engine.torch_mod()
+    if x.dim() == 1:
+      x = x.unsqueeze(0)
+    if x.dtype != torch.float32 or x.dim() != 2 or x.device.type != "cuda":
+      raise ValueError("x must be a CUDA float32 tensor [streams, samples]")
+    S, T = x.shape
+    L = self.order + 1
+    with torch.cuda.device(x.device):
+      if state is None:
+        state = self.new_state(S)
+      self._check_state(state, S, x.device)
+      if x.stride(1) != 1:
+        x = x.contiguous()
+      xs = x.stride(0) if S > 1 else max(T, 1)     # a length-1 axis may carry any stride
+      F = self.n_frames(state.consumed, T, final)
+      dev = x.device
+      w = self._window(dev)
+      stream = torch.cuda.current_stream(dev).cuda_stream
+      if levinson:
+        coef = torch.empty((S, F, L), dtype=torch.float64, device=dev)
+        err = torch.empty((S, F), dtype=torch.float64, device=dev)
+        failed = torch.empty((S, F), dtype=torch.uint8, device=dev)
+        nbytes = _check(lib().alz_lpc_scratch_bytes(S, F, self.order))
+        scratch = torch.empty(max(8, nbytes), dtype=torch.uint8, device=dev)   # on this stream: torch's allocator orders reuse
+        _check(lib().alz_lpc_apply_f32(x.data_ptr(), xs, None if w is None else w.data_ptr(), None, coef.data_ptr(),
+                                       err.data_ptr(), failed.data_ptr(), F, state.tensor.data_ptr(), S, T, self.order,
+                                       self.size, self.hop, int(bool(final)), scratch.data_ptr(), nbytes, stream))
+        out = LpcResult(coef, err, failed)
+      else:
+        out = torch.empty((S, F, L), dtype=torch.float64, device=dev)
+        _check(lib().alz_lpc_apply_f32(x.data_ptr(), xs, None if w is None else w.data_ptr(), out.data_ptr(), None,
+                                       None, None, F, state.tensor.data_ptr(), S, T, self.order, self.size, self.hop,
+                                       int(bool(final)), None, 0, stream))
+    state.consumed += T
+    state.ended = bool(final)
+    return out
+
+  def apply(self, x, state=None, final=False):
+    """Coefficients, squared prediction errors and failure flags of every frame this call emits."""
+    return self._run(x, state, final, True)
+
+  def acorr(self, x, state=None, final=False):
+    """Autocorrelation lags 0 .. order of every frame this call emits."""
+    return self._run(x, state, final, False)
+
+
+def lpc_frames(seq, order, size, hop=None, window=None):
+  """Lazy Stream of the analysis filters of every block of ``Stream(seq).blocks(size, hop)`` (times ``window``, when
+  given): element ``k`` is the reference's ``lpc.kautocor(block k, order)``, a FIR :class:`ZFilter` with the squared
+  prediction error in ``.error``, bit for bit.  Reaching a frame where the reference raises :class:`ParCorError`
+  raises it, after the frames before it."""
+  lp = LpcFrames(order, size, hop, window)
+  torch = _engine.torch_mod()
+  state = lp.new_state(1)                          # no device: raises at call time
+  device = state.device
+
+  def frames(res):
+    coef, err, failed = (t[0].cpu().numpy() for t in res)
+    for c, e, f in zip(coef, err, failed):
+      if f:
+        raise ParCorError("Can't find next PARCOR coefficient")
+      filt = ZFilter([1] + c[1:].tolist())
+      filt.error = float(e)
+      yield filt
+
+  def pump():
+    for xb in _engine._blocks(seq):
+      yield frames(lp.apply(torch.from_numpy(xb).to(device), state=state))
+    yield frames(lp.apply(torch.empty((1, 0), dtype=torch.float32, device=device), state=state, final=True))
+
+  return Stream(it.chain.from_iterable(pump()))
