@@ -3,14 +3,18 @@
 ``nvcc`` cross-compiles for sm_90a (H100) without a GPU; the built ``.so`` files are git-ignored
 but travel to the GPU box with the repository snapshot.
 
-* ``libalz_b200.so``, the filter library: the translation units ``csrc/*.cu`` (the C ABI plus
-  one unit of kernel instantiations per cascade length) are compiled in parallel into
-  ``_native/obj/`` and linked into ONE shared library.
-* ``libalz_b200_amdf.so``, the AMDF library: ``csrc_amdf/*.cu`` behind ``include/alz_b200_amdf.h``,
-  compiled with ``-fmad=false`` (its float64 arithmetic reproduces AudioLazy's bit for bit).
+:data:`LIBRARIES` lists the four libraries.  Each one is the ``.cu`` units of its source directory, compiled in
+parallel into ``_native/obj/<name>/`` (only the units that changed) and linked into one shared library:
+
+* ``libalz_b200.so``, the filter library: ``csrc/*.cu`` behind ``include/alz_b200.h`` (the C ABI plus one unit of
+  kernel instantiations per cascade length).
+* ``libalz_b200_amdf.so``, the AMDF library: ``csrc_amdf/*.cu`` behind ``include/alz_b200_amdf.h``, compiled with
+  ``-fmad=false`` (its float64 arithmetic reproduces AudioLazy's bit for bit).
 * ``libalz_b200_zcross.so``, the zero-crossing library: ``csrc_zcross/*.cu`` behind ``include/alz_b200_zcross.h``.
 * ``libalz_b200_lpc.so``, the frame-wise LPC library: ``csrc_lpc/*.cu`` behind ``include/alz_b200_lpc.h``, compiled
   with ``-fmad=false`` (its float64 sums reproduce AudioLazy's bit for bit).
+
+The three analysis libraries also include ``csrc_common/alz_common.h``.
 """
 from __future__ import annotations
 
@@ -18,48 +22,65 @@ import os
 import shutil
 import subprocess
 from concurrent.futures import ThreadPoolExecutor
+from typing import NamedTuple
 
-_PKG = os.path.dirname(os.path.abspath(__file__))
-CSRC = os.path.join(_PKG, "csrc")
-NATIVE_DIR = os.path.join(_PKG, "_native")
-OBJ_DIR = os.path.join(NATIVE_DIR, "obj")
-LIB_PATH = os.path.join(NATIVE_DIR, "libalz_b200.so")
-INCLUDE = os.path.join(os.path.dirname(_PKG), "include")
-AMDF_CSRC = os.path.join(_PKG, "csrc_amdf")
-AMDF_LIB_PATH = os.path.join(NATIVE_DIR, "libalz_b200_amdf.so")
-AMDF_HEADER = os.path.join(INCLUDE, "alz_b200_amdf.h")
-ZCROSS_CSRC = os.path.join(_PKG, "csrc_zcross")
-ZCROSS_LIB_PATH = os.path.join(NATIVE_DIR, "libalz_b200_zcross.so")
-ZCROSS_HEADER = os.path.join(INCLUDE, "alz_b200_zcross.h")
-LPC_CSRC = os.path.join(_PKG, "csrc_lpc")
-LPC_LIB_PATH = os.path.join(NATIVE_DIR, "libalz_b200_lpc.so")
-LPC_HEADER = os.path.join(INCLUDE, "alz_b200_lpc.h")
+#: the repository root, which the paths of :data:`LIBRARIES` are resolved against when they are used
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+PKG = "audiolazy_b200"
+NATIVE = os.path.join(PKG, "_native")
 
 ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH_FLAGS + [
   "-O3", "-lineinfo", "-std=c++17",
-  "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",   # only the extern "C" ABI of include/alz_b200.h is exported
+  "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",   # only the extern "C" ABI of the public header is exported
 ]
 
 
-def _units():
-  return sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith(".cu"))
+class Library(NamedTuple):
+  """One shared library, ``_native/<file>``.  Every ``.cu`` of the package directory ``csrc`` is a unit; every
+  ``.cuh`` / ``.h`` there, the public ``include/<header>`` and the private headers ``deps`` (package paths) are
+  dependencies of all of them.  ``flags`` are added to the nvcc flags of its units."""
+  name: str
+  file: str
+  csrc: str
+  header: str
+  flags: tuple = ()
+  deps: tuple = ()
+
+  @property
+  def path(self):
+    return os.path.join(ROOT, NATIVE, self.file)
+
+  def units(self):
+    d = os.path.join(ROOT, PKG, self.csrc)
+    return sorted(os.path.join(d, f) for f in os.listdir(d) if f.endswith(".cu"))
+
+  def headers(self):
+    d = os.path.join(ROOT, PKG, self.csrc)
+    return sorted(os.path.join(d, f) for f in os.listdir(d) if f.endswith((".cuh", ".h"))) + \
+           [os.path.join(ROOT, "include", self.header)] + [os.path.join(ROOT, PKG, h) for h in self.deps]
 
 
-def _headers():
-  return sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))) + \
-         [os.path.join(INCLUDE, "alz_b200.h")]
+_COMMON = ("csrc_common/alz_common.h",)
+LIBRARIES = {lib.name: lib for lib in (
+  Library("filters", "libalz_b200.so", "csrc", "alz_b200.h"),
+  Library("amdf", "libalz_b200_amdf.so", "csrc_amdf", "alz_b200_amdf.h", ("-fmad=false",), _COMMON),
+  Library("zcross", "libalz_b200_zcross.so", "csrc_zcross", "alz_b200_zcross.h", (), _COMMON),
+  Library("lpc", "libalz_b200_lpc.so", "csrc_lpc", "alz_b200_lpc.h", ("-fmad=false",), _COMMON),
+)}
+#: the filter library (``_capi`` loads it from here unless ``ALZ_B200_LIB`` names another file)
+LIB_PATH = LIBRARIES["filters"].path
+AMDF_LIB_PATH = LIBRARIES["amdf"].path
+ZCROSS_LIB_PATH = LIBRARIES["zcross"].path
+LPC_LIB_PATH = LIBRARIES["lpc"].path
 
 
-def _sources():
-  return _units() + _headers()
-
-
-def is_stale() -> bool:
-  if not os.path.exists(LIB_PATH):
+def is_stale(lib: Library) -> bool:
+  """The library is missing or older than one of its sources."""
+  if not os.path.exists(lib.path):
     return True
-  t = os.path.getmtime(LIB_PATH)
-  return any(os.path.getmtime(s) > t for s in _sources())
+  t = os.path.getmtime(lib.path)
+  return any(os.path.getmtime(s) > t for s in lib.units() + lib.headers())
 
 
 def find_nvcc():
@@ -67,108 +88,36 @@ def find_nvcc():
   return nvcc if os.path.exists(nvcc) else None
 
 
-def build_native(force: bool = False, verbose: bool = False) -> str:
-  """Build the four libraries (see :func:`build_filters`, :func:`build_amdf`, :func:`build_zcross` and
-  :func:`build_lpc`); returns the filter library's path."""
-  path = build_filters(force=force, verbose=verbose)
-  build_amdf(force=force, verbose=verbose)
-  build_zcross(force=force, verbose=verbose)
-  build_lpc(force=force, verbose=verbose)
-  return path
+def build_native(force: bool = False, verbose: bool = False) -> list:
+  """Build every library of :data:`LIBRARIES`; returns their paths."""
+  return [build_library(lib, force=force, verbose=verbose) for lib in LIBRARIES.values()]
 
 
-def _amdf_sources():
-  return sorted(os.path.join(AMDF_CSRC, f) for f in os.listdir(AMDF_CSRC) if f.endswith((".cu", ".cuh", ".h"))) + \
-         [AMDF_HEADER]
-
-
-def build_amdf(force: bool = False, verbose: bool = False) -> str:
-  """Compile ``csrc_amdf/*.cu`` for sm_90a with ``-fmad=false`` and link ``libalz_b200_amdf.so``."""
-  if not force and os.path.exists(AMDF_LIB_PATH) and \
-     all(os.path.getmtime(s) <= os.path.getmtime(AMDF_LIB_PATH) for s in _amdf_sources()):
-    return AMDF_LIB_PATH
+def build_library(lib: Library, force: bool = False, verbose: bool = False) -> str:
+  """Compile the units of ``lib`` that changed for sm_90a, in parallel, and link its shared library."""
+  if not force and not is_stale(lib):
+    return lib.path
   nvcc = find_nvcc()
   if nvcc is None:
-    raise RuntimeError("nvcc not found: cannot build audiolazy_b200's AMDF library")
-  os.makedirs(NATIVE_DIR, exist_ok=True)
-  units = sorted(os.path.join(AMDF_CSRC, f) for f in os.listdir(AMDF_CSRC) if f.endswith(".cu"))
-  tmp = AMDF_LIB_PATH + ".tmp.%d" % os.getpid()
-  cmd = [nvcc] + NVCC_FLAGS + ["-fmad=false"] + (["-Xptxas", "-v"] if verbose else []) + ["-shared", "-o", tmp] + units
-  subprocess.check_call(cmd)
-  os.replace(tmp, AMDF_LIB_PATH)
-  return AMDF_LIB_PATH
-
-
-def _zcross_sources():
-  return sorted(os.path.join(ZCROSS_CSRC, f) for f in os.listdir(ZCROSS_CSRC) if f.endswith((".cu", ".cuh", ".h"))) + \
-         [ZCROSS_HEADER]
-
-
-def build_zcross(force: bool = False, verbose: bool = False) -> str:
-  """Compile ``csrc_zcross/*.cu`` for sm_90a and link ``libalz_b200_zcross.so``."""
-  if not force and os.path.exists(ZCROSS_LIB_PATH) and \
-     all(os.path.getmtime(s) <= os.path.getmtime(ZCROSS_LIB_PATH) for s in _zcross_sources()):
-    return ZCROSS_LIB_PATH
-  nvcc = find_nvcc()
-  if nvcc is None:
-    raise RuntimeError("nvcc not found: cannot build audiolazy_b200's zero-crossing library")
-  os.makedirs(NATIVE_DIR, exist_ok=True)
-  units = sorted(os.path.join(ZCROSS_CSRC, f) for f in os.listdir(ZCROSS_CSRC) if f.endswith(".cu"))
-  tmp = ZCROSS_LIB_PATH + ".tmp.%d" % os.getpid()
-  cmd = [nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-shared", "-o", tmp] + units
-  subprocess.check_call(cmd)
-  os.replace(tmp, ZCROSS_LIB_PATH)
-  return ZCROSS_LIB_PATH
-
-
-def _lpc_sources():
-  return sorted(os.path.join(LPC_CSRC, f) for f in os.listdir(LPC_CSRC) if f.endswith((".cu", ".cuh", ".h"))) + \
-         [LPC_HEADER]
-
-
-def build_lpc(force: bool = False, verbose: bool = False) -> str:
-  """Compile ``csrc_lpc/*.cu`` for sm_90a with ``-fmad=false`` and link ``libalz_b200_lpc.so``."""
-  if not force and os.path.exists(LPC_LIB_PATH) and \
-     all(os.path.getmtime(s) <= os.path.getmtime(LPC_LIB_PATH) for s in _lpc_sources()):
-    return LPC_LIB_PATH
-  nvcc = find_nvcc()
-  if nvcc is None:
-    raise RuntimeError("nvcc not found: cannot build audiolazy_b200's LPC library")
-  os.makedirs(NATIVE_DIR, exist_ok=True)
-  units = sorted(os.path.join(LPC_CSRC, f) for f in os.listdir(LPC_CSRC) if f.endswith(".cu"))
-  tmp = LPC_LIB_PATH + ".tmp.%d" % os.getpid()
-  cmd = [nvcc] + NVCC_FLAGS + ["-fmad=false"] + (["-Xptxas", "-v"] if verbose else []) + ["-shared", "-o", tmp] + units
-  subprocess.check_call(cmd)
-  os.replace(tmp, LPC_LIB_PATH)
-  return LPC_LIB_PATH
-
-
-def build_filters(force: bool = False, verbose: bool = False) -> str:
-  """Compile ``csrc/*.cu`` for sm_90a (only the units that changed) and link the filter library."""
-  if not force and not is_stale():
-    return LIB_PATH
-  nvcc = find_nvcc()
-  if nvcc is None:
-    raise RuntimeError("nvcc not found: cannot build audiolazy_b200's CUDA library")
-  os.makedirs(OBJ_DIR, exist_ok=True)
-  newest_header = max(os.path.getmtime(h) for h in _headers())
-  jobs = []
-  for src in _units():
-    obj = os.path.join(OBJ_DIR, os.path.splitext(os.path.basename(src))[0] + ".o")
-    if force or not os.path.exists(obj) or os.path.getmtime(obj) < max(os.path.getmtime(src), newest_header):
-      jobs.append((src, obj))
+    raise RuntimeError("nvcc not found: cannot build audiolazy_b200's %s" % lib.file)
+  obj_dir = os.path.join(ROOT, NATIVE, "obj", lib.name)
+  os.makedirs(obj_dir, exist_ok=True)
+  newest_header = max(os.path.getmtime(h) for h in lib.headers())
+  units = lib.units()
+  objs = [os.path.join(obj_dir, os.path.splitext(os.path.basename(src))[0] + ".o") for src in units]
+  jobs = [(src, obj) for src, obj in zip(units, objs)
+          if force or not os.path.exists(obj) or os.path.getmtime(obj) < max(os.path.getmtime(src), newest_header)]
 
   def compile_one(job):
     src, obj = job
     tmp = obj + ".tmp.%d" % os.getpid()
-    cmd = [nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-c", "-o", tmp, src]
+    cmd = [nvcc] + NVCC_FLAGS + list(lib.flags) + (["-Xptxas", "-v"] if verbose else []) + ["-c", "-o", tmp, src]
     subprocess.check_call(cmd)
     os.replace(tmp, obj)
 
   with ThreadPoolExecutor(max_workers=max(1, min(len(jobs), os.cpu_count() or 1))) as pool:
     list(pool.map(compile_one, jobs))
-  objs = [os.path.join(OBJ_DIR, os.path.splitext(os.path.basename(s))[0] + ".o") for s in _units()]
-  tmp = LIB_PATH + ".tmp.%d" % os.getpid()
+  tmp = lib.path + ".tmp.%d" % os.getpid()
   subprocess.check_call([nvcc] + ARCH_FLAGS + ["-shared", "-o", tmp] + objs)
-  os.replace(tmp, LIB_PATH)
-  return LIB_PATH
+  os.replace(tmp, lib.path)
+  return lib.path

@@ -28,19 +28,55 @@ PLAN_DESIGN_ONLY = 4
 PLAN_SEQUENTIAL = 8
 PLAN_PARALLEL = 16
 
-#: every symbol include/alz_b200.h declares (tests check the library exports them all)
-SYMBOLS = (
-  "alz_last_error", "alz_abi_version", "alz_device_count", "alz_set_device", "alz_plan_create", "alz_plan_create_ex",
-  "alz_plan_destroy", "alz_plan_taps", "alz_apply_tv_f32", "alz_plan_tiers", "alz_apply_f32_ex", "alz_host_alloc",
-  "alz_host_free", "alz_stream_create_partition", "alz_stream_destroy_partition", "alz_apply_sum_f32", "alz_apply_envelope_f32", "alz_apply_envelope_f32_host",
-  "alz_apply_envelope_f32_ex", "alz_apply_envelope_f32_host_ex",
-  "alz_plan_info_get", "alz_plan_state_doubles", "alz_state_init", "alz_plan_history", "alz_apply_f32",
-  "alz_apply_f32_host", "alz_sum_channels_f32", "alz_freq_response_f64", "alz_launch_count",
-)
-
 
 class NativeError(RuntimeError):
   """The native CUDA library is missing or a native call failed."""
+
+
+class NativeLib(object):
+  """The ctypes binding of one of the package's native libraries.
+
+  ``prototypes`` maps every function the library's header declares to its ``(restype, argtypes)``; :attr:`symbols`
+  is that list.  :meth:`load` opens the library once (``path``, or the file the environment variable ``env`` names)
+  and binds the prototypes.  :meth:`check` turns a negative status code into the exception ``errors`` maps it to
+  (called with the message of the library's ``*_last_error`` function), or into a :class:`NativeError`."""
+
+  def __init__(self, path, name, prototypes, errors, env=None):
+    self.path = path
+    self.name = name
+    self.prototypes = prototypes
+    self.symbols = tuple(prototypes)
+    self.errors = errors
+    self.env = env
+    self.last_error = next(s for s in prototypes if s.endswith("_last_error"))
+    self.cdll = None
+
+  def load(self, reload=False):
+    """Load the library once (again with ``reload``); raise :class:`NativeError` if it is absent or cannot be loaded."""
+    if self.cdll is not None and not reload:
+      return self.cdll
+    path = os.environ.get(self.env, self.path) if self.env else self.path
+    if not os.path.exists(path):
+      raise NativeError(
+        "audiolazy_b200 %s library not found at %s -- build it with "
+        "`python -c 'import __graft_entry__ as g; g.build()'` (there is no CPU fallback)" % (self.name, path))
+    try:
+      L = ctypes.CDLL(path)
+    except OSError as exc:
+      raise NativeError("cannot load %s: %s" % (path, exc))
+    for symbol, (restype, argtypes) in self.prototypes.items():
+      fn = getattr(L, symbol)
+      fn.restype, fn.argtypes = restype, argtypes
+    self.cdll = L
+    return L
+
+  def check(self, rc):
+    if rc < 0:
+      msg = getattr(self.load(), self.last_error)().decode("utf-8", "replace")
+      if rc in self.errors:
+        raise self.errors[rc](msg)
+      raise NativeError("%s error %d: %s" % (self.last_error[:-len("_last_error")], rc, msg))
+    return rc
 
 
 class PlanInfo(ctypes.Structure):
@@ -49,93 +85,58 @@ class PlanInfo(ctypes.Structure):
                "device", "n_fp32_channels", "tier_tol_e9")] + [("reserved", ctypes.c_int32 * 5)]
 
 
+_i32, _i64, _f64, _vp, _p = ctypes.c_int32, ctypes.c_int64, ctypes.c_double, ctypes.c_void_p, ctypes.POINTER
+LIB = NativeLib(_build.LIB_PATH, "native", {
+  "alz_last_error": (ctypes.c_char_p, []),
+  "alz_abi_version": (_i32, []),
+  "alz_device_count": (_i32, []),
+  "alz_set_device": (_i32, [_i32]),
+  "alz_plan_create": (_i32, [_vp, _vp, _i32, _i32, _p(_vp)]),
+  "alz_plan_create_ex": (_i32, [_vp, _vp, _i32, _i32, _i32, _p(_vp)]),
+  "alz_plan_destroy": (None, [_vp]),
+  "alz_plan_taps": (_i32, [_vp, _vp, _vp, _i32]),
+  "alz_plan_tiers": (_i32, [_vp, _vp, _vp, _i32]),
+  "alz_plan_info_get": (_i32, [_vp, _p(PlanInfo)]),
+  "alz_plan_state_doubles": (_i64, [_vp, _i64]),
+  "alz_state_init": (_i32, [_vp, _vp, _i64, _vp, _vp, _vp]),
+  "alz_plan_history": (_i32, [_vp, _p(_i32), _p(_i32)]),
+  "alz_apply_f32": (_i32, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _i64, _vp]),
+  "alz_apply_f32_ex": (_i32, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _i64, _i64, _vp]),
+  "alz_apply_tv_f32": (_i32, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _i64, _vp, _i64, _vp]),
+  "alz_apply_sum_f32": (_i32, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _i64, _vp]),
+  "alz_apply_envelope_f32": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _i64, _i32, _i32, _f64, _f64, _vp]),
+  "alz_apply_envelope_f32_host": (_i32, [_vp, _vp, _vp, _i64, _i64, _i64, _i64, _i32, _i32, _f64, _f64]),
+  "alz_apply_envelope_f32_ex": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _i64, _i32, _i32, _i32, _f64, _f64,
+                                       _vp]),
+  "alz_apply_envelope_f32_host_ex": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _i64, _i32, _i32, _i32, _f64,
+                                            _f64]),
+  "alz_stream_create_partition": (_i32, [_i32, _i32, _p(_vp), _p(_i32)]),
+  "alz_stream_destroy_partition": (_i32, [_vp]),
+  "alz_host_alloc": (_i32, [_p(_vp), _i64, _i32, _p(_i32)]),
+  "alz_host_free": (_i32, [_vp]),
+  "alz_apply_f32_host": (_i32, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _i64]),
+  "alz_sum_channels_f32": (_i32, [_vp, _vp, _i64, _i32, _i64, _i64, _i64, _vp]),
+  "alz_freq_response_f64": (_i32, [_vp, _vp, _vp, _i64, _vp]),
+  "alz_launch_count": (_i64, []),
+}, {
+  ALZ_ERR_ZERO_GAIN: lambda msg: ZeroDivisionError("Invalid filter gain"),   # same exception as lazy_filters.py:177-178
+  ALZ_ERR_INVALID: ValueError,
+}, env="ALZ_B200_LIB")
+#: every function include/alz_b200.h declares
+SYMBOLS = LIB.symbols
+_check = LIB.check
+#: the loaded filter library; None until :func:`lib` loads it, and setting it back to None makes the next call load it
+#: again (from the file ``ALZ_B200_LIB`` names then)
 _lib = None
 
 
 def lib():
-  """Load (once) ``_native/libalz_b200.so``; raise :class:`NativeError` if absent."""
+  """Load (once) ``_native/libalz_b200.so``, or the file ``ALZ_B200_LIB`` names; raise :class:`NativeError` if it
+  cannot be loaded."""
   global _lib
-  if _lib is not None:
-    return _lib
-  path = os.environ.get("ALZ_B200_LIB", _build.LIB_PATH)
-  if not os.path.exists(path):
-    raise NativeError(
-      "audiolazy_b200 native library not found at %s -- build it with "
-      "`python -c 'import __graft_entry__ as g; g.build()'` (there is no CPU fallback)" % path)
-  try:
-    L = ctypes.CDLL(path)
-  except OSError as exc:  # pragma: no cover
-    raise NativeError("cannot load %s: %s" % (path, exc))
-  i32, i64, vp = ctypes.c_int32, ctypes.c_int64, ctypes.c_void_p
-  L.alz_last_error.restype = ctypes.c_char_p
-  L.alz_last_error.argtypes = []
-  L.alz_abi_version.restype = i32
-  L.alz_device_count.restype = i32
-  L.alz_set_device.restype = i32
-  L.alz_set_device.argtypes = [i32]
-  L.alz_plan_create.restype = i32
-  L.alz_plan_create.argtypes = [vp, vp, i32, i32, ctypes.POINTER(vp)]
-  L.alz_plan_create_ex.restype = i32
-  L.alz_plan_create_ex.argtypes = [vp, vp, i32, i32, i32, ctypes.POINTER(vp)]
-  L.alz_plan_taps.restype = i32
-  L.alz_plan_taps.argtypes = [vp, vp, vp, i32]
-  L.alz_plan_tiers.restype = i32
-  L.alz_plan_tiers.argtypes = [vp, vp, vp, i32]
-  L.alz_apply_tv_f32.restype = i32
-  L.alz_apply_tv_f32.argtypes = [vp, vp, vp, vp, i64, i64, i64, i64, vp, i64, vp]
-  L.alz_plan_destroy.restype = None
-  L.alz_plan_destroy.argtypes = [vp]
-  L.alz_plan_info_get.restype = i32
-  L.alz_plan_info_get.argtypes = [vp, ctypes.POINTER(PlanInfo)]
-  L.alz_plan_state_doubles.restype = i64
-  L.alz_plan_state_doubles.argtypes = [vp, i64]
-  L.alz_state_init.restype = i32
-  L.alz_state_init.argtypes = [vp, vp, i64, vp, vp, vp]
-  L.alz_plan_history.restype = i32
-  L.alz_plan_history.argtypes = [vp, ctypes.POINTER(i32), ctypes.POINTER(i32)]
-  L.alz_apply_f32.restype = i32
-  L.alz_apply_f32.argtypes = [vp, vp, vp, vp, i64, i64, i64, i64, vp]
-  L.alz_apply_f32_ex.restype = i32
-  L.alz_apply_f32_ex.argtypes = [vp, vp, vp, vp, i64, i64, i64, i64, i64, vp]
-  L.alz_apply_sum_f32.restype = i32
-  L.alz_apply_sum_f32.argtypes = [vp, vp, vp, vp, i64, i64, i64, i64, vp]
-  f64 = ctypes.c_double
-  L.alz_apply_envelope_f32.restype = i32
-  L.alz_apply_envelope_f32.argtypes = [vp, vp, vp, vp, vp, i64, i64, i64, i64, i32, i32, f64, f64, vp]
-  L.alz_apply_envelope_f32_host.restype = i32
-  L.alz_apply_envelope_f32_host.argtypes = [vp, vp, vp, i64, i64, i64, i64, i32, i32, f64, f64]
-  L.alz_apply_envelope_f32_ex.restype = i32
-  L.alz_apply_envelope_f32_ex.argtypes = [vp, vp, vp, vp, vp, i64, i64, i64, i64, i32, i32, i32, f64, f64, vp]
-  L.alz_apply_envelope_f32_host_ex.restype = i32
-  L.alz_apply_envelope_f32_host_ex.argtypes = [vp, vp, vp, vp, vp, i64, i64, i64, i64, i32, i32, i32, f64, f64]
-  L.alz_stream_create_partition.restype = i32
-  L.alz_stream_create_partition.argtypes = [i32, i32, ctypes.POINTER(vp), ctypes.POINTER(i32)]
-  L.alz_stream_destroy_partition.restype = i32
-  L.alz_stream_destroy_partition.argtypes = [vp]
-  L.alz_host_alloc.restype = i32
-  L.alz_host_alloc.argtypes = [ctypes.POINTER(vp), i64, i32, ctypes.POINTER(i32)]
-  L.alz_host_free.restype = i32
-  L.alz_host_free.argtypes = [vp]
-  L.alz_apply_f32_host.restype = i32
-  L.alz_apply_f32_host.argtypes = [vp, vp, vp, vp, i64, i64, i64, i64]
-  L.alz_sum_channels_f32.restype = i32
-  L.alz_sum_channels_f32.argtypes = [vp, vp, i64, i32, i64, i64, i64, vp]
-  L.alz_freq_response_f64.restype = i32
-  L.alz_freq_response_f64.argtypes = [vp, vp, vp, i64, vp]
-  L.alz_launch_count.restype = i64
-  _lib = L
-  return L
-
-
-def _check(rc):
-  if rc < 0:
-    msg = lib().alz_last_error().decode("utf-8", "replace")
-    if rc == ALZ_ERR_ZERO_GAIN:
-      raise ZeroDivisionError("Invalid filter gain")   # same exception as lazy_filters.py:177-178
-    if rc == ALZ_ERR_INVALID:
-      raise ValueError(msg)
-    raise NativeError("alz error %d: %s" % (rc, msg))
-  return rc
+  if _lib is None:
+    _lib = LIB.load(reload=True)
+  return _lib
 
 
 def pack_sections(bank):

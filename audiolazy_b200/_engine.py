@@ -32,6 +32,42 @@ def torch_mod():
   return torch
 
 
+def stream_input(x):
+  """The input of a batched call: a CUDA float32 tensor ``x[streams, samples]`` (1-D: one stream) ->
+  ``(x, S, T, row_stride)``, its rows made contiguous."""
+  torch = torch_mod()
+  if x.dim() == 1:
+    x = x.unsqueeze(0)
+  if x.dtype != torch.float32 or x.dim() != 2 or x.device.type != "cuda":
+    raise ValueError("x must be a CUDA float32 tensor [streams, samples]")
+  if x.stride(1) != 1:
+    x = x.contiguous()
+  S, T = x.shape
+  return x, S, T, x.stride(0) if S > 1 else max(T, 1)     # a length-1 axis may carry any stride
+
+
+def check_state(state, cls, owner, S, device):
+  """The checks every streaming state takes before its own: ``state`` is a ``cls`` (from ``<owner>.new_state``) made
+  for ``S`` streams on ``device``."""
+  if not isinstance(state, cls):
+    raise ValueError("state must come from %s.new_state" % owner)
+  if state.n_streams != S:
+    raise ValueError("state was created for %d streams, x has %d" % (state.n_streams, S))
+  if state.device != device:
+    raise ValueError("state lives on %s, x on %s" % (state.device, device))
+
+
+def n_blocks(consumed, T, size, hop, final):
+  """Blocks of ``Stream(x).blocks(size, hop)`` a call on ``T`` samples emits after ``consumed`` samples: the blocks it
+  completes, plus, with ``final``, the padded last block when the reference emits one (``alz_lpc_frames``)."""
+  ka = max(0, (consumed - size) // hop + 1)
+  kc = (consumed + T - size) // hop
+  n = max(0, kc - ka + 1)
+  if final and consumed + T - max(kc + 1, 0) * hop > max(size - hop, 0):
+    n += 1
+  return n
+
+
 def _key(bank_sections):
   return tuple(tuple((tuple(b), tuple(a)) for b, a in channel) for channel in bank_sections)
 

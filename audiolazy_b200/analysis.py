@@ -9,7 +9,6 @@ device and continued block by block through an :class:`AmdfState`.  ``amdf`` is 
 from __future__ import annotations
 
 import ctypes
-import os
 from numbers import Integral
 
 import numpy as np
@@ -21,49 +20,20 @@ __all__ = ["amdf", "AmdfBank", "AmdfState"]
 
 PLAN_SEQUENTIAL = 8
 
+_i32, _i64, _f64, _vp = ctypes.c_int32, ctypes.c_int64, ctypes.c_double, ctypes.c_void_p
+LIB = _capi.NativeLib(_build.AMDF_LIB_PATH, "AMDF", {
+  "alz_amdf_last_error": (ctypes.c_char_p, []),
+  "alz_amdf_plan_create": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, ctypes.POINTER(_vp)]),
+  "alz_amdf_plan_destroy": (None, [_vp]),
+  "alz_amdf_state_doubles": (_i64, [_vp, _i64]),
+  "alz_amdf_state_init": (_i32, [_vp, _vp, _i64, _f64, _vp]),
+  "alz_amdf_plan_chunks": (_i64, [_vp, _i64, _i64]),
+  "alz_amdf_apply_f32": (_i32, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _i64, _i32, _i32, _vp]),
+}, {_capi.ALZ_ERR_INVALID: ValueError, _capi.ALZ_ERR_NONCAUSAL: ValueError})
 #: every function include/alz_b200_amdf.h declares
-SYMBOLS = ("alz_amdf_last_error", "alz_amdf_plan_create", "alz_amdf_plan_destroy", "alz_amdf_state_doubles",
-           "alz_amdf_state_init", "alz_amdf_plan_chunks", "alz_amdf_apply_f32")
-
-_lib = None
-
-
-def lib():
-  """Load (once) ``_native/libalz_b200_amdf.so``; raise :class:`~audiolazy_b200._capi.NativeError` if absent."""
-  global _lib
-  if _lib is not None:
-    return _lib
-  path = _build.AMDF_LIB_PATH
-  if not os.path.exists(path):
-    raise _capi.NativeError("audiolazy_b200 AMDF library not found at %s -- build it with "
-                            "`python -c 'import __graft_entry__ as g; g.build()'` (there is no CPU fallback)" % path)
-  L = ctypes.CDLL(path)
-  i32, i64, vp, f64 = ctypes.c_int32, ctypes.c_int64, ctypes.c_void_p, ctypes.c_double
-  L.alz_amdf_last_error.restype = ctypes.c_char_p
-  L.alz_amdf_last_error.argtypes = []
-  L.alz_amdf_plan_create.restype = i32
-  L.alz_amdf_plan_create.argtypes = [vp, vp, vp, i32, i32, i32, ctypes.POINTER(vp)]
-  L.alz_amdf_plan_destroy.restype = None
-  L.alz_amdf_plan_destroy.argtypes = [vp]
-  L.alz_amdf_state_doubles.restype = i64
-  L.alz_amdf_state_doubles.argtypes = [vp, i64]
-  L.alz_amdf_state_init.restype = i32
-  L.alz_amdf_state_init.argtypes = [vp, vp, i64, f64, vp]
-  L.alz_amdf_plan_chunks.restype = i64
-  L.alz_amdf_plan_chunks.argtypes = [vp, i64, i64]
-  L.alz_amdf_apply_f32.restype = i32
-  L.alz_amdf_apply_f32.argtypes = [vp, vp, vp, vp, i64, i64, i64, i64, i32, i32, vp]
-  _lib = L
-  return L
-
-
-def _check(rc):
-  if rc < 0:
-    msg = lib().alz_amdf_last_error().decode("utf-8", "replace")
-    if rc in (_capi.ALZ_ERR_INVALID, _capi.ALZ_ERR_NONCAUSAL):
-      raise ValueError(msg)
-    raise _capi.NativeError("alz_amdf error %d: %s" % (rc, msg))
-  return rc
+SYMBOLS = LIB.symbols
+lib = LIB.load
+_check = LIB.check
 
 
 def lag_taps(lag):
@@ -108,8 +78,8 @@ class _Plan(object):
 
   def __del__(self):
     h, self._h = getattr(self, "_h", None), None
-    if h and _lib is not None:
-      _lib.alz_amdf_plan_destroy(h)
+    if h and LIB.cdll is not None:
+      LIB.cdll.alz_amdf_plan_destroy(h)
 
   def state_doubles(self, n_streams):
     return _check(lib().alz_amdf_state_doubles(self._h, int(n_streams)))
@@ -196,24 +166,15 @@ class AmdfBank(object):
     return self._plan().chunks(n_streams, n_samples)
 
   def _check_state(self, state, n_streams, decim, device):
-    if not isinstance(state, AmdfState):
-      raise ValueError("state must come from AmdfBank.new_state")
+    _engine.check_state(state, AmdfState, "AmdfBank", n_streams, device)
     if not self._same(state.bank):
       raise ValueError("state belongs to another bank")
-    if state.n_streams != n_streams:
-      raise ValueError("state was created for %d streams, x has %d" % (state.n_streams, n_streams))
-    if state.device != device:
-      raise ValueError("state lives on %s, x on %s" % (state.device, device))
     if state.decim != int(decim):
       raise ValueError("state was created for decim=%d, the call asks for decim=%r" % (state.decim, decim))
 
   def apply(self, x, decim=1, state=None):
     torch = _engine.torch_mod()
-    if x.dim() == 1:
-      x = x.unsqueeze(0)
-    if x.dtype != torch.float32 or x.dim() != 2 or x.device.type != "cuda":
-      raise ValueError("x must be a CUDA float32 tensor [streams, samples]")
-    S, T = x.shape
+    x, S, T, xs = _engine.stream_input(x)
     if int(decim) < 1:
       raise ValueError("decim must be >= 1")
     with torch.cuda.device(x.device):
@@ -221,11 +182,8 @@ class AmdfBank(object):
       if state is None:
         state = self.new_state(S, decim=decim)
       self._check_state(state, S, decim, x.device)
-      if x.stride(1) != 1:
-        x = x.contiguous()
       n_out = (state.phase + T) // state.decim
       out = torch.empty((S, len(self), n_out), dtype=torch.float32, device=x.device)
-      xs = x.stride(0) if S > 1 else max(T, 1)     # a length-1 axis may carry any stride
       plan.apply(x.data_ptr(), out.data_ptr(), state.tensor.data_ptr(), S, T, xs, max(n_out, 1), state.decim, state.phase,
                  torch.cuda.current_stream(x.device).cuda_stream)
     state.phase = (state.phase + T) % state.decim

@@ -11,53 +11,27 @@ from __future__ import annotations
 import ctypes
 import itertools as it
 import math
-import os
 from numbers import Integral, Real
 
 from . import _build, _capi, _engine
+from ._engine import n_blocks
 from .stream import Stream
 
 __all__ = ["zcross", "Zcross", "ZcrossState"]
 
+_i32, _i64, _f64, _vp = ctypes.c_int32, ctypes.c_int64, ctypes.c_double, ctypes.c_void_p
+LIB = _capi.NativeLib(_build.ZCROSS_LIB_PATH, "zero-crossing", {
+  "alz_zcross_last_error": (ctypes.c_char_p, []),
+  "alz_zcross_state_bytes": (_i64, [_i64, _i32, _i32]),
+  "alz_zcross_state_init": (_i32, [_vp, _i64, _f64, _i32, _i32, _vp]),
+  "alz_zcross_scratch_bytes": (_i64, [_i64, _i64, _i32, _i32]),
+  "alz_zcross_apply_f32": (_i32, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _i64, _i32, _i32, _f64, _i32, _vp, _i64,
+                                  _vp]),
+}, {_capi.ALZ_ERR_INVALID: ValueError})
 #: every function include/alz_b200_zcross.h declares
-SYMBOLS = ("alz_zcross_last_error", "alz_zcross_state_bytes", "alz_zcross_state_init", "alz_zcross_scratch_bytes",
-           "alz_zcross_apply_f32")
-
-_lib = None
-
-
-def lib():
-  """Load (once) ``_native/libalz_b200_zcross.so``; raise :class:`~audiolazy_b200._capi.NativeError` if absent."""
-  global _lib
-  if _lib is not None:
-    return _lib
-  path = _build.ZCROSS_LIB_PATH
-  if not os.path.exists(path):
-    raise _capi.NativeError("audiolazy_b200 zero-crossing library not found at %s -- build it with "
-                            "`python -c 'import __graft_entry__ as g; g.build()'` (there is no CPU fallback)" % path)
-  L = ctypes.CDLL(path)
-  i32, i64, vp, f64 = ctypes.c_int32, ctypes.c_int64, ctypes.c_void_p, ctypes.c_double
-  L.alz_zcross_last_error.restype = ctypes.c_char_p
-  L.alz_zcross_last_error.argtypes = []
-  L.alz_zcross_state_bytes.restype = i64
-  L.alz_zcross_state_bytes.argtypes = [i64, i32, i32]
-  L.alz_zcross_state_init.restype = i32
-  L.alz_zcross_state_init.argtypes = [vp, i64, f64, i32, i32, vp]
-  L.alz_zcross_scratch_bytes.restype = i64
-  L.alz_zcross_scratch_bytes.argtypes = [i64, i64, i32, i32]
-  L.alz_zcross_apply_f32.restype = i32
-  L.alz_zcross_apply_f32.argtypes = [vp, i64, vp, i64, vp, i64, vp, i64, i64, i32, i32, f64, i32, vp, i64, vp]
-  _lib = L
-  return L
-
-
-def _check(rc):
-  if rc < 0:
-    msg = lib().alz_zcross_last_error().decode("utf-8", "replace")
-    if rc == _capi.ALZ_ERR_INVALID:
-      raise ValueError(msg)
-    raise _capi.NativeError("alz_zcross error %d: %s" % (rc, msg))
-  return rc
+SYMBOLS = LIB.symbols
+lib = LIB.load
+_check = LIB.check
 
 
 def _real(name, value):
@@ -77,16 +51,6 @@ def _block_arg(name, value):
   if value < 1:
     raise ValueError("%s must be >= 1 (got %d)" % (name, value))
   return int(value)
-
-
-def n_blocks(consumed, T, size, hop, final):
-  """Counts one call stores (``include/alz_b200_zcross.h``): the blocks it completes, plus the padded last block."""
-  ka = max(0, (consumed - size) // hop + 1)
-  kc = (consumed + T - size) // hop
-  n = max(0, kc - ka + 1)
-  if final and consumed + T - max(kc + 1, 0) * hop > max(size - hop, 0):
-    n += 1
-  return n
 
 
 class ZcrossState(object):
@@ -138,15 +102,10 @@ class Zcross(object):
     return ZcrossState(self, n_streams, size=size, hop=hop)
 
   def _check_state(self, state, S, size, hop, device):
-    if not isinstance(state, ZcrossState):
-      raise ValueError("state must come from Zcross.new_state")
+    _engine.check_state(state, ZcrossState, "Zcross", S, device)
     same_h = state.hysteresis == self.hysteresis or (math.isnan(state.hysteresis) and math.isnan(self.hysteresis))
     if not same_h or state.sign != self.sign:
       raise ValueError("state belongs to a Zcross with another hysteresis or first_sign")
-    if state.n_streams != S:
-      raise ValueError("state was created for %d streams, x has %d" % (state.n_streams, S))
-    if state.device != device:
-      raise ValueError("state lives on %s, x on %s" % (state.device, device))
     if (state.size, state.hop) != (size, hop):
       raise ValueError("state was created for size=%r, hop=%r; the call asks for size=%r, hop=%r"
                        % (state.size, state.hop, size, hop))
@@ -155,18 +114,11 @@ class Zcross(object):
 
   def _run(self, x, state, size, hop, final, flags):
     torch = _engine.torch_mod()
-    if x.dim() == 1:
-      x = x.unsqueeze(0)
-    if x.dtype != torch.float32 or x.dim() != 2 or x.device.type != "cuda":
-      raise ValueError("x must be a CUDA float32 tensor [streams, samples]")
-    S, T = x.shape
+    x, S, T, xs = _engine.stream_input(x)
     with torch.cuda.device(x.device):
       if state is None:
         state = self.new_state(S, size=size, hop=hop)
       self._check_state(state, S, size, hop, x.device)
-      if x.stride(1) != 1:
-        x = x.contiguous()
-      xs = x.stride(0) if S > 1 else max(T, 1)     # a length-1 axis may carry any stride
       out = torch.empty((S, T), dtype=torch.uint8, device=x.device) if flags else None
       nb = n_blocks(state.consumed, T, size, hop, final) if size else 0
       counts = torch.empty((S, nb), dtype=torch.int32, device=x.device) if size else None

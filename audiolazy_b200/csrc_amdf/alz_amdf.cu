@@ -14,17 +14,15 @@
 #pragma GCC visibility push(default)
 #include "../../include/alz_b200_amdf.h"
 #pragma GCC visibility pop
+#include "../csrc_common/alz_common.h"
 
 #include <cuda_runtime.h>
 
 #include <algorithm>
 #include <cmath>
-#include <cstdarg>
-#include <cstdio>
 #include <cstdlib>
 #include <mutex>
 #include <set>
-#include <string>
 #include <vector>
 
 namespace {
@@ -61,24 +59,6 @@ struct AmdfPlan {
   double inv;
   AmdfLag* d_lags;
 };
-
-thread_local std::string g_err;
-
-int fail(int code, const char* fmt, ...) {
-  char buf[512];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof buf, fmt, ap);
-  va_end(ap);
-  g_err = buf;
-  return code;
-}
-
-#define AMDF_CUDA(call)                                                                              \
-  do {                                                                                              \
-    cudaError_t e_ = (call);                                                                        \
-    if (e_ != cudaSuccess) return fail(ALZ_AMDF_ERR_CUDA, "%s: %s", #call, cudaGetErrorString(e_)); \
-  } while (0)
 
 bool env_flag(const char* name) {
   const char* v = getenv(name);
@@ -365,7 +345,7 @@ int32_t alz_amdf_state_init(const void* plan, double* state_dev, int64_t n_strea
   const long long sstride = 2 + (long long)p->H + 2 * (long long)p->L, n = n_streams * sstride;
   const unsigned blocks = (unsigned)std::min<long long>((n + 255) / 256, 4096);
   alz_amdf_init_kernel<<<blocks, 256, 0, (cudaStream_t)cuda_stream>>>(state_dev, n, sstride, zero);
-  AMDF_CUDA(cudaGetLastError());
+  ALZ_CUDA_CHECK(cudaGetLastError(), ALZ_AMDF_ERR_CUDA);
   return ALZ_AMDF_OK;
 }
 
@@ -388,7 +368,7 @@ int32_t alz_amdf_apply_f32(const void* plan, const float* x_dev, float* out_dev,
   if (n_streams > 1 && x_stride < n_samples) return fail(ALZ_AMDF_ERR_INVALID, "x_stride < n_samples");
   if ((n_streams > 1 || p->L > 1) && out_stride < n_out) return fail(ALZ_AMDF_ERR_INVALID, "out_stride < n_out");
   int dev = -1;
-  AMDF_CUDA(cudaGetDevice(&dev));
+  ALZ_CUDA_CHECK(cudaGetDevice(&dev), ALZ_AMDF_ERR_CUDA);
   if (dev != p->device) return fail(ALZ_AMDF_ERR_INVALID, "the plan lives on device %d, device %d is current", p->device, dev);
   const long long P = chunks(p, n_streams, n_samples);
   if (n_streams * P * p->n_groups > 0x7fffffffLL || n_streams > 0x7fffffffLL)
@@ -414,9 +394,9 @@ int32_t alz_amdf_apply_f32(const void* plan, const float* x_dev, float* out_dev,
   a.inv = p->inv;
   const cudaStream_t st = (cudaStream_t)cuda_stream;
   alz_amdf_kernel<<<(unsigned)(n_streams * P * p->n_groups), kThreads, p->smem, st>>>(a);
-  AMDF_CUDA(cudaGetLastError());
+  ALZ_CUDA_CHECK(cudaGetLastError(), ALZ_AMDF_ERR_CUDA);
   alz_amdf_commit_kernel<<<(unsigned)n_streams, 256, 0, st>>>(a);
-  AMDF_CUDA(cudaGetLastError());
+  ALZ_CUDA_CHECK(cudaGetLastError(), ALZ_AMDF_ERR_CUDA);
   return ALZ_AMDF_OK;
 }
 

@@ -15,14 +15,12 @@
 #pragma GCC visibility push(default)
 #include "../../include/alz_b200_lpc.h"
 #pragma GCC visibility pop
+#include "../csrc_common/alz_common.h"
 
 #include <cuda_runtime.h>
 
 #include <cmath>
-#include <cstdarg>
 #include <cstdint>
-#include <cstdio>
-#include <string>
 
 namespace {
 
@@ -42,33 +40,6 @@ struct LpcArgs {
   long long xs, sstride, T, F;
   int order, size, hop, final_, fpc, blocks_per_stream;
 };
-
-thread_local std::string g_err;
-
-int fail(int code, const char* fmt, ...) {
-  char buf[512];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof buf, fmt, ap);
-  va_end(ap);
-  g_err = buf;
-  return code;
-}
-
-#define LPC_CUDA(call)                                                                              \
-  do {                                                                                              \
-    cudaError_t e_ = (call);                                                                        \
-    if (e_ != cudaSuccess) return fail(ALZ_LPC_ERR_CUDA, "%s: %s", #call, cudaGetErrorString(e_));  \
-  } while (0)
-
-__host__ __device__ inline long long floordiv(long long a, long long b) {   // b > 0
-  return a >= 0 ? a / b : -((-a + b - 1) / b);
-}
-
-__host__ __device__ inline long long first_open_frame(long long n, int size, int hop) {   // first k: k hop + size > n
-  const long long k = floordiv(n - size, hop) + 1;
-  return k > 0 ? k : 0;
-}
 
 long long state_stride(int size) { return (16 + 4 * (long long)size + 7) / 8 * 8; }
 
@@ -110,7 +81,7 @@ __global__ void __launch_bounds__(kMaxFramesPerCta * 32) alz_lpc_kernel(const __
   const long long C = *reinterpret_cast<const long long*>(st);
   const float* tail = reinterpret_cast<const float*>(st + 16);    // samples [C - size, C)
   const float* xr = a.x + s * a.xs;
-  const long long ka = first_open_frame(C, a.size, a.hop);
+  const long long ka = first_open_block(C, a.size, a.hop);
   const int size = a.size, ld = size + 1;
   const int nf = (int)(a.F - i0 < a.fpc ? a.F - i0 : a.fpc);
 
@@ -260,12 +231,7 @@ const char* alz_lpc_last_error(void) { return g_err.c_str(); }
 int64_t alz_lpc_frames(int64_t consumed, int64_t n_samples, int32_t size, int32_t hop, int32_t final) {
   if (consumed < 0 || n_samples < 0 || size < 1 || hop < 1)
     return fail(ALZ_LPC_ERR_INVALID, "need consumed >= 0, n_samples >= 0, size >= 1, hop >= 1");
-  const long long ka = first_open_frame(consumed, size, hop);
-  const long long kc = floordiv(consumed + n_samples - size, hop);
-  long long n = kc - ka + 1 > 0 ? kc - ka + 1 : 0;
-  const long long kp = kc + 1 > 0 ? kc + 1 : 0;
-  if (final && consumed + n_samples - kp * hop > (size > hop ? size - hop : 0)) ++n;
-  return n;
+  return emitted_blocks(consumed, n_samples, size, hop, final != 0);
 }
 
 int64_t alz_lpc_state_bytes(int64_t n_streams, int32_t size) {
@@ -282,7 +248,7 @@ int32_t alz_lpc_state_init(void* state_dev, int64_t n_streams, int32_t size, voi
   const long long n = n_streams * (state_stride(size) / 4);
   const unsigned blocks = (unsigned)((n + kThreadsCommit - 1) / kThreadsCommit < 4096 ? (n + kThreadsCommit - 1) / kThreadsCommit : 4096);
   alz_lpc_init_kernel<<<blocks, kThreadsCommit, 0, (cudaStream_t)cuda_stream>>>((unsigned char*)state_dev, n);
-  LPC_CUDA(cudaGetLastError());
+  ALZ_CUDA_CHECK(cudaGetLastError(), ALZ_LPC_ERR_CUDA);
   return ALZ_LPC_OK;
 }
 
@@ -340,21 +306,23 @@ int32_t alz_lpc_apply_f32(const float* x_dev, int64_t x_stride, const double* wi
     if (grid > 0x7fffffffLL || n_frames > 0x7fffffffLL) return fail(ALZ_LPC_ERR_UNSUPPORTED, "too many frames for one launch");
     const int threads = (a.fpc * (order + 1) + 31) / 32 * 32;
     const size_t smem = (size_t)a.fpc * (size + 1) * 8;
-    if (smem > 48 * 1024) LPC_CUDA(cudaFuncSetAttribute(alz_lpc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if (smem > 48 * 1024)
+      ALZ_CUDA_CHECK(cudaFuncSetAttribute(alz_lpc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
+                     ALZ_LPC_ERR_CUDA);
     alz_lpc_kernel<<<(unsigned)grid, threads, smem, cs>>>(a);
-    LPC_CUDA(cudaGetLastError());
+    ALZ_CUDA_CHECK(cudaGetLastError(), ALZ_LPC_ERR_CUDA);
     if (levinson) {
       const long long total = n_streams * n_frames;
       const int nt = levinson_threads(order);
       const long long blocks = (total + nt - 1) / nt;
       if (blocks > 0x7fffffffLL) return fail(ALZ_LPC_ERR_UNSUPPORTED, "too many frames for one launch");
       alz_lpc_levinson_kernel<<<(unsigned)blocks, nt, (size_t)2 * 8 * (order + 1) * nt, cs>>>(a, total);
-      LPC_CUDA(cudaGetLastError());
+      ALZ_CUDA_CHECK(cudaGetLastError(), ALZ_LPC_ERR_CUDA);
     }
   }
   if (n_samples > 0) {
     alz_lpc_commit_kernel<<<(unsigned)n_streams, kThreadsCommit, (size_t)4 * size, cs>>>(a);
-    LPC_CUDA(cudaGetLastError());
+    ALZ_CUDA_CHECK(cudaGetLastError(), ALZ_LPC_ERR_CUDA);
   }
   return ALZ_LPC_OK;
 }

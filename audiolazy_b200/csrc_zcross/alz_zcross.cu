@@ -20,14 +20,12 @@
 #pragma GCC visibility push(default)
 #include "../../include/alz_b200_zcross.h"
 #pragma GCC visibility pop
+#include "../csrc_common/alz_common.h"
 
 #include <cuda_runtime.h>
 
 #include <cmath>
-#include <cstdarg>
 #include <cstdint>
-#include <cstdio>
-#include <string>
 
 namespace {
 
@@ -49,33 +47,6 @@ struct ZcArgs {
   int size, hop, R, final_;
   float hf;
 };
-
-thread_local std::string g_err;
-
-int fail(int code, const char* fmt, ...) {
-  char buf[512];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof buf, fmt, ap);
-  va_end(ap);
-  g_err = buf;
-  return code;
-}
-
-#define ZC_CUDA(call)                                                                                  \
-  do {                                                                                                \
-    cudaError_t e_ = (call);                                                                          \
-    if (e_ != cudaSuccess) return fail(ALZ_ZCROSS_ERR_CUDA, "%s: %s", #call, cudaGetErrorString(e_)); \
-  } while (0)
-
-__host__ __device__ inline long long floordiv(long long a, long long b) {   // b > 0
-  return a >= 0 ? a / b : -((-a + b - 1) / b);
-}
-
-__host__ __device__ inline long long first_open_block(long long n, int size, int hop) {   // first k with k hop + size > n
-  const long long k = floordiv(n - size, hop) + 1;
-  return k > 0 ? k : 0;
-}
 
 long long ring_slots(int size, int hop) { return size > 0 ? (size + (long long)hop - 1) / hop : 0; }
 
@@ -345,7 +316,7 @@ int32_t alz_zcross_state_init(void* state_dev, int64_t n_streams, double first_s
   const unsigned blocks = (unsigned)((n + kThreads - 1) / kThreads < 4096 ? (n + kThreads - 1) / kThreads : 4096);
   alz_zcross_init_kernel<<<blocks, kThreads, 0, (cudaStream_t)cuda_stream>>>((unsigned char*)state_dev, n_streams,
                                                                             state_stride(size, hop), sign);
-  ZC_CUDA(cudaGetLastError());
+  ALZ_CUDA_CHECK(cudaGetLastError(), ALZ_ZCROSS_ERR_CUDA);
   return ALZ_ZCROSS_OK;
 }
 
@@ -398,13 +369,14 @@ int32_t alz_zcross_apply_f32(const float* x_dev, int64_t x_stride, uint8_t* flag
     if ((double)a.hf > hysteresis) a.hf = std::nextafter(a.hf, -INFINITY);
   }
   const cudaStream_t cs = (cudaStream_t)cuda_stream;
-  ZC_CUDA(cudaMemsetAsync(scratch_dev, 0, (size_t)alz_zcross_scratch_bytes(n_streams, n_samples, size, hop), cs));
+  ALZ_CUDA_CHECK(cudaMemsetAsync(scratch_dev, 0, (size_t)alz_zcross_scratch_bytes(n_streams, n_samples, size, hop), cs),
+                 ALZ_ZCROSS_ERR_CUDA);
   if (nt > 0) {
     alz_zcross_kernel<<<(unsigned)(n_streams * nt), kThreads, 0, cs>>>(a);
-    ZC_CUDA(cudaGetLastError());
+    ALZ_CUDA_CHECK(cudaGetLastError(), ALZ_ZCROSS_ERR_CUDA);
   }
   alz_zcross_finish_kernel<<<(unsigned)n_streams, kThreads, 0, cs>>>(a);
-  ZC_CUDA(cudaGetLastError());
+  ALZ_CUDA_CHECK(cudaGetLastError(), ALZ_ZCROSS_ERR_CUDA);
   return ALZ_ZCROSS_OK;
 }
 

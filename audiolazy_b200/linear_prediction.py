@@ -20,12 +20,10 @@ import cmath
 import collections
 import ctypes
 import itertools as it
-import os
 from numbers import Integral, Real
 
 from . import _build, _capi, _engine
 from .core import StrategyDict
-from .crossing import n_blocks
 from .filters import ZFilter
 from .stream import Stream
 
@@ -248,49 +246,23 @@ def lsf_stable(filt):
 # Frame-wise LPC on the GPU (include/alz_b200_lpc.h)
 # ---------------------------------------------------------------------------------------------------------------------
 
-#: every function include/alz_b200_lpc.h declares
-SYMBOLS = ("alz_lpc_last_error", "alz_lpc_frames", "alz_lpc_state_bytes", "alz_lpc_state_init", "alz_lpc_scratch_bytes",
-           "alz_lpc_apply_f32")
 MAX_ORDER = 64
 MAX_SIZE = 8192
 
-_lib = None
-
-
-def lib():
-  """Load (once) ``_native/libalz_b200_lpc.so``; raise :class:`~audiolazy_b200._capi.NativeError` if absent."""
-  global _lib
-  if _lib is not None:
-    return _lib
-  path = _build.LPC_LIB_PATH
-  if not os.path.exists(path):
-    raise _capi.NativeError("audiolazy_b200 LPC library not found at %s -- build it with "
-                            "`python -c 'import __graft_entry__ as g; g.build()'` (there is no CPU fallback)" % path)
-  L = ctypes.CDLL(path)
-  i32, i64, vp = ctypes.c_int32, ctypes.c_int64, ctypes.c_void_p
-  L.alz_lpc_last_error.restype = ctypes.c_char_p
-  L.alz_lpc_last_error.argtypes = []
-  L.alz_lpc_frames.restype = i64
-  L.alz_lpc_frames.argtypes = [i64, i64, i32, i32, i32]
-  L.alz_lpc_state_bytes.restype = i64
-  L.alz_lpc_state_bytes.argtypes = [i64, i32]
-  L.alz_lpc_state_init.restype = i32
-  L.alz_lpc_state_init.argtypes = [vp, i64, i32, vp]
-  L.alz_lpc_scratch_bytes.restype = i64
-  L.alz_lpc_scratch_bytes.argtypes = [i64, i64, i32]
-  L.alz_lpc_apply_f32.restype = i32
-  L.alz_lpc_apply_f32.argtypes = [vp, i64, vp, vp, vp, vp, vp, i64, vp, i64, i64, i32, i32, i32, i32, vp, i64, vp]
-  _lib = L
-  return L
-
-
-def _check(rc):
-  if rc < 0:
-    msg = lib().alz_lpc_last_error().decode("utf-8", "replace")
-    if rc == _capi.ALZ_ERR_INVALID:
-      raise ValueError(msg)
-    raise _capi.NativeError("alz_lpc error %d: %s" % (rc, msg))
-  return rc
+_i32, _i64, _vp = ctypes.c_int32, ctypes.c_int64, ctypes.c_void_p
+LIB = _capi.NativeLib(_build.LPC_LIB_PATH, "LPC", {
+  "alz_lpc_last_error": (ctypes.c_char_p, []),
+  "alz_lpc_frames": (_i64, [_i64, _i64, _i32, _i32, _i32]),
+  "alz_lpc_state_bytes": (_i64, [_i64, _i32]),
+  "alz_lpc_state_init": (_i32, [_vp, _i64, _i32, _vp]),
+  "alz_lpc_scratch_bytes": (_i64, [_i64, _i64, _i32]),
+  "alz_lpc_apply_f32": (_i32, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _i64, _i64, _i32, _i32, _i32, _i32, _vp,
+                               _i64, _vp]),
+}, {_capi.ALZ_ERR_INVALID: ValueError})
+#: every function include/alz_b200_lpc.h declares
+SYMBOLS = LIB.symbols
+lib = LIB.load
+_check = LIB.check
 
 
 def _int_arg(name, value, lo, hi):
@@ -369,7 +341,7 @@ class LpcFrames(object):
 
   def n_frames(self, consumed, T, final):
     """Frames a call on ``T`` samples emits after ``consumed`` samples (the block count of ``zcross``'s counts)."""
-    return n_blocks(consumed, T, self.size, self.hop, final)
+    return _engine.n_blocks(consumed, T, self.size, self.hop, final)
 
   def _window(self, device):
     if self.window is None:
@@ -381,32 +353,20 @@ class LpcFrames(object):
     return w
 
   def _check_state(self, state, S, device):
-    if not isinstance(state, LpcState):
-      raise ValueError("state must come from LpcFrames.new_state")
+    _engine.check_state(state, LpcState, "LpcFrames", S, device)
     if state.key != self._key():
       raise ValueError("state belongs to an LpcFrames with another order, size, hop or window")
-    if state.n_streams != S:
-      raise ValueError("state was created for %d streams, x has %d" % (state.n_streams, S))
-    if state.device != device:
-      raise ValueError("state lives on %s, x on %s" % (state.device, device))
     if state.ended:
       raise ValueError("state was ended by a call with final=True")
 
   def _run(self, x, state, final, levinson):
     torch = _engine.torch_mod()
-    if x.dim() == 1:
-      x = x.unsqueeze(0)
-    if x.dtype != torch.float32 or x.dim() != 2 or x.device.type != "cuda":
-      raise ValueError("x must be a CUDA float32 tensor [streams, samples]")
-    S, T = x.shape
+    x, S, T, xs = _engine.stream_input(x)
     L = self.order + 1
     with torch.cuda.device(x.device):
       if state is None:
         state = self.new_state(S)
       self._check_state(state, S, x.device)
-      if x.stride(1) != 1:
-        x = x.contiguous()
-      xs = x.stride(0) if S > 1 else max(T, 1)     # a length-1 axis may carry any stride
       F = self.n_frames(state.consumed, T, final)
       dev = x.device
       w = self._window(dev)

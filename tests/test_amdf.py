@@ -5,9 +5,6 @@ import builtins
 import json
 import math
 import os
-import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -15,7 +12,8 @@ import pytest
 import audiolazy_b200 as ab
 from audiolazy_b200 import _build, analysis as amdf_mod
 from amdf_emulation import amdf as emulate, digest
-from conftest import GOLDEN, ROOT
+from conftest import GOLDEN
+from native_libs import check_exports, check_sm90a
 
 
 @pytest.fixture(scope="module")
@@ -85,25 +83,9 @@ def test_freq2lag_lag2freq():
   assert ab.freq2lag(2 * math.pi / 37.25) == 2 * math.pi / (2 * math.pi / 37.25)
 
 
-def header_functions():
-  text = open(os.path.join(ROOT, "include", "alz_b200_amdf.h")).read()
-  text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
-  return sorted(set(re.findall(r"\b(alz_[a-z0-9_]+)\s*\(", text)))
-
-
 def test_amdf_library_exports_exactly_its_header():
-  assert os.path.exists(_build.AMDF_LIB_PATH), "run `python -c 'import __graft_entry__ as g; g.build()'` first"
-  declared = header_functions()
-  assert sorted(amdf_mod.SYMBOLS) == declared
-  if not shutil.which("nm"):
-    pytest.skip("nm not available")
-  out = subprocess.run(["nm", "-D", "--defined-only", _build.AMDF_LIB_PATH], capture_output=True, text=True).stdout
-  assert sorted(line.split()[-1] for line in out.splitlines() if " T alz_" in line) == declared
+  check_exports(amdf_mod.LIB, "alz_b200_amdf.h")
 
 
 def test_amdf_library_is_sm90a():
-  cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-  if not os.path.exists(cuobjdump):
-    pytest.skip("cuobjdump not available")
-  out = subprocess.run([cuobjdump, "-lelf", _build.AMDF_LIB_PATH], capture_output=True, text=True).stdout
-  assert "sm_90a" in out
+  check_sm90a(_build.AMDF_LIB_PATH)

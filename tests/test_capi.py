@@ -1,6 +1,5 @@
 """The C-ABI shared library: builds, loads, exports every symbol include/alz_b200.h
 declares, and fails loudly (never silently falls back) without a CUDA device."""
-import ctypes
 import os
 import re
 
@@ -9,12 +8,7 @@ import pytest
 
 from audiolazy_b200 import _build, _capi
 from conftest import ROOT
-
-
-def header_functions():
-  text = open(os.path.join(ROOT, "include", "alz_b200.h")).read()
-  text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
-  return sorted(set(re.findall(r"\b(alz_[a-z0-9_]+)\s*\(", text)))
+from native_libs import check_exports, check_sm90a, cuobjdump, header_functions
 
 
 def test_library_is_built_in_tree():
@@ -23,31 +17,16 @@ def test_library_is_built_in_tree():
 
 
 def test_exports_every_declared_symbol():
-  lib = ctypes.CDLL(_build.LIB_PATH)
-  declared = header_functions()
-  assert len(declared) >= 14
-  for name in declared:
-    assert hasattr(lib, name), "library does not export %s" % name
-  assert sorted(_capi.SYMBOLS) == declared           # the Python binding covers the whole ABI
-  import shutil
-  import subprocess
-  if shutil.which("nm"):                             # ... and nothing else with the prefix leaks out of the library
-    out = subprocess.run(["nm", "-D", "--defined-only", _build.LIB_PATH], capture_output=True, text=True).stdout
-    exported = sorted(line.split()[-1] for line in out.splitlines() if " T alz_" in line)
-    assert exported == declared
+  assert len(header_functions("alz_b200.h")) >= 14
   assert _capi.lib().alz_abi_version() == 2
+  check_exports(_capi.LIB, "alz_b200.h")
 
 
 def test_sass_is_sm90a_with_fp64_and_uniform_operands():
-  import shutil
   import subprocess
-  cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-  if not os.path.exists(cuobjdump):
-    pytest.skip("cuobjdump not available")
-  out = subprocess.run([cuobjdump, "-lelf", _build.LIB_PATH], capture_output=True, text=True).stdout
-  assert "sm_90a" in out
+  check_sm90a(_build.LIB_PATH)
   # stream the SASS and stop as soon as both signatures have been seen
-  proc = subprocess.Popen([cuobjdump, "-sass", _build.LIB_PATH], stdout=subprocess.PIPE, text=True)
+  proc = subprocess.Popen([cuobjdump(), "-sass", _build.LIB_PATH], stdout=subprocess.PIPE, text=True)
   seen_ur = seen_cp = seen_tma_ld = seen_tma_st = False
   for line in proc.stdout:
     seen_ur = seen_ur or re.search(r"DFMA R\d+, R\d+(\.reuse)?, UR\d+, R\d+", line) is not None

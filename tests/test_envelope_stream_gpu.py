@@ -8,20 +8,12 @@ from scipy.signal import lfilter
 
 import audiolazy_b200 as ab
 from conftest import GOLDEN, rel_err, signal
+from native_libs import torch  # noqa: F401  (fixture)
 
 pytestmark = pytest.mark.gpu
 
 STRATEGIES = ["slaney", "klapuri", "sampled"]
 MODES = ["abs", "squared", "rms"]
-
-
-@pytest.fixture(scope="module")
-def torch():
-  torch = pytest.importorskip("torch")
-  if not torch.cuda.is_available():
-    pytest.skip("no CUDA device")
-  torch.cuda.set_device(0)
-  return torch
 
 
 _BANKS = {}

@@ -17,14 +17,13 @@ Tolerances (max |y - oracle| / max |oracle| per output row):
 import contextlib
 import os
 import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
 import oracle
 from conftest import rel_err
+from native_libs import compiled_kernels
 
 TIER0_GAIN_IN = 2.5e-7
 TIER0 = 6.5e-8
@@ -695,15 +694,7 @@ def kernel_key(name):
 
 def library_kernels():
   from audiolazy_b200 import _build
-  cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-  filt = shutil.which("c++filt") or shutil.which("cu++filt") or "/usr/local/cuda/bin/cu++filt"
-  if not (os.path.exists(cuobjdump) and os.path.exists(filt)):
-    pytest.skip("cuobjdump / c++filt not available")
-  elf = subprocess.run([cuobjdump, "-elf", _build.LIB_PATH], capture_output=True, text=True, check=True).stdout
-  mangled = sorted(set(re.findall(r"\.text\.(_Z\w+)", elf)))
-  assert mangled, "no kernels found in %s" % _build.LIB_PATH
-  demangled = subprocess.run([filt], input="\n".join(mangled), capture_output=True, text=True, check=True).stdout
-  keys = {kernel_key(n) for n in demangled.splitlines()}
+  keys = {kernel_key(n) for n in compiled_kernels(_build.LIB_PATH)}
   assert None not in keys
   return keys
 

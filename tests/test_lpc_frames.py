@@ -5,7 +5,6 @@ import json
 import math
 import os
 import re
-import shutil
 import subprocess
 import sys
 
@@ -14,7 +13,8 @@ import pytest
 
 import audiolazy_b200 as ab
 from audiolazy_b200 import _build, crossing, linear_prediction as lp
-from conftest import GOLDEN, ROOT
+from conftest import GOLDEN
+from native_libs import check_exports, check_sm90a, cuobjdump
 import lpc_emulation as em
 
 sys.path.insert(0, GOLDEN)
@@ -117,38 +117,18 @@ def test_library_sizes_without_a_device():
   assert "order" in L.alz_lpc_last_error().decode()
 
 
-def header_functions():
-  text = open(os.path.join(ROOT, "include", "alz_b200_lpc.h")).read()
-  text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
-  return sorted(set(re.findall(r"\b(alz_[a-z0-9_]+)\s*\(", text)))
-
-
 def test_lpc_library_exports_exactly_its_header():
-  assert os.path.exists(_build.LPC_LIB_PATH), "run `python -c 'import __graft_entry__ as g; g.build()'` first"
-  declared = header_functions()
-  assert sorted(lp.SYMBOLS) == declared
-  if not shutil.which("nm"):
-    pytest.skip("nm not available")
-  out = subprocess.run(["nm", "-D", "--defined-only", _build.LPC_LIB_PATH], capture_output=True, text=True).stdout
-  assert sorted(line.split()[-1] for line in out.splitlines() if " T alz_" in line) == declared
-
-
-def _cuobjdump():
-  cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-  if not os.path.exists(cuobjdump):
-    pytest.skip("cuobjdump not available")
-  return cuobjdump
+  check_exports(lp.LIB, "alz_b200_lpc.h")
 
 
 def test_lpc_library_is_sm90a():
-  out = subprocess.run([_cuobjdump(), "-lelf", _build.LPC_LIB_PATH], capture_output=True, text=True).stdout
-  assert "sm_90a" in out
+  check_sm90a(_build.LPC_LIB_PATH)
 
 
 def test_lpc_library_has_no_fused_multiply_add():
   """Built with -fmad=false: no product is contracted into an add, as the reference's arithmetic requires.  The only
   DFMAs are the Newton steps of the one correctly rounded division in the Levinson-Durbin kernel (c = num / den)."""
-  sass = subprocess.run([_cuobjdump(), "-sass", _build.LPC_LIB_PATH], capture_output=True, text=True).stdout
+  sass = subprocess.run([cuobjdump(), "-sass", _build.LPC_LIB_PATH], capture_output=True, text=True).stdout
   functions = re.split(r"\n\s*Function : ", sass)[1:]
   assert len(functions) == 4
   by_name = {f.split(None, 1)[0]: f for f in functions}

@@ -1,0 +1,59 @@
+"""Every native library of ``_build.LIBRARIES``: it has a Python binding, that binding fails loudly when the library
+cannot be loaded (there is no CPU fallback), and the library is rebuilt when a source it depends on changes.  Each
+library's exports, target and kernel launches are checked next to its other tests (``native_libs.check_*``)."""
+import os
+import shutil
+
+import pytest
+
+from audiolazy_b200 import _build, _capi, analysis, crossing, linear_prediction
+from conftest import ROOT
+
+NAMES = sorted(_build.LIBRARIES)
+BINDINGS = {"filters": _capi.LIB, "amdf": analysis.LIB, "zcross": crossing.LIB, "lpc": linear_prediction.LIB}
+
+
+def test_every_library_has_a_binding():
+  assert sorted(BINDINGS) == NAMES
+
+
+@pytest.mark.parametrize("name", NAMES)
+def test_unloadable_library_raises_native_error(name, tmp_path, monkeypatch):
+  """A missing file and a file that is not a shared library both raise NativeError, never a silent fallback."""
+  binding = BINDINGS[name]
+  monkeypatch.delenv("ALZ_B200_LIB", raising=False)
+  monkeypatch.setattr(binding, "cdll", None)
+  monkeypatch.setattr(binding, "path", str(tmp_path / "missing.so"))
+  with pytest.raises(_capi.NativeError, match="no CPU fallback"):
+    binding.load()
+  junk = tmp_path / "junk.so"
+  junk.write_text("not an ELF file\n")
+  monkeypatch.setattr(binding, "path", str(junk))
+  with pytest.raises(_capi.NativeError, match="cannot load"):
+    binding.load()
+
+
+def test_staleness_follows_the_dependencies(tmp_path, monkeypatch):
+  """In a copy of the sources: touching the shared header marks exactly the three analysis libraries stale, touching
+  one library's unit or public header marks only that library stale."""
+  for d in ("include", "audiolazy_b200"):
+    shutil.copytree(os.path.join(ROOT, d), str(tmp_path / d), ignore=shutil.ignore_patterns("_native", "__pycache__"))
+  monkeypatch.setattr(_build, "ROOT", str(tmp_path))
+  libs = list(_build.LIBRARIES.values())
+  os.makedirs(str(tmp_path / _build.NATIVE))
+  for lib in libs:
+    open(lib.path, "w").close()
+
+  def stale_after_touching(rel):
+    for lib in libs:
+      for src in lib.units() + lib.headers():
+        os.utime(src, (1000, 1000))
+      os.utime(lib.path, (2000, 2000))
+    assert not any(_build.is_stale(lib) for lib in libs)
+    os.utime(str(tmp_path / rel), (3000, 3000))
+    return sorted(lib.name for lib in libs if _build.is_stale(lib))
+
+  assert stale_after_touching("audiolazy_b200/csrc_common/alz_common.h") == ["amdf", "lpc", "zcross"]
+  assert stale_after_touching("audiolazy_b200/csrc_lpc/alz_lpc.cu") == ["lpc"]
+  assert stale_after_touching("include/alz_b200_zcross.h") == ["zcross"]
+  assert stale_after_touching("audiolazy_b200/csrc/alz_plan.h") == ["filters"]

@@ -4,9 +4,6 @@ import ast
 import json
 import math
 import os
-import re
-import shutil
-import subprocess
 import sys
 
 import numpy as np
@@ -14,7 +11,8 @@ import pytest
 
 import audiolazy_b200 as ab
 from audiolazy_b200 import _build, crossing
-from conftest import GOLDEN, ROOT
+from conftest import GOLDEN
+from native_libs import check_exports, check_sm90a
 from zcross_emulation import block_sums, digest, zcross as emulate
 
 sys.path.insert(0, GOLDEN)
@@ -97,28 +95,12 @@ def test_n_blocks_matches_the_emulated_split(consumed, T, size, hop, final):
   assert crossing.n_blocks(consumed, T, size, hop, final) == total - before
 
 
-def header_functions():
-  text = open(os.path.join(ROOT, "include", "alz_b200_zcross.h")).read()
-  text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
-  return sorted(set(re.findall(r"\b(alz_[a-z0-9_]+)\s*\(", text)))
-
-
 def test_zcross_library_exports_exactly_its_header():
-  assert os.path.exists(_build.ZCROSS_LIB_PATH), "run `python -c 'import __graft_entry__ as g; g.build()'` first"
-  declared = header_functions()
-  assert sorted(crossing.SYMBOLS) == declared
-  if not shutil.which("nm"):
-    pytest.skip("nm not available")
-  out = subprocess.run(["nm", "-D", "--defined-only", _build.ZCROSS_LIB_PATH], capture_output=True, text=True).stdout
-  assert sorted(line.split()[-1] for line in out.splitlines() if " T alz_" in line) == declared
+  check_exports(crossing.LIB, "alz_b200_zcross.h")
 
 
 def test_zcross_library_is_sm90a():
-  cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-  if not os.path.exists(cuobjdump):
-    pytest.skip("cuobjdump not available")
-  out = subprocess.run([cuobjdump, "-lelf", _build.ZCROSS_LIB_PATH], capture_output=True, text=True).stdout
-  assert "sm_90a" in out
+  check_sm90a(_build.ZCROSS_LIB_PATH)
 
 
 def test_library_sizes_without_a_device():

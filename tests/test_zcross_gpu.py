@@ -5,9 +5,6 @@ import itertools as it
 import json
 import math
 import os
-import re
-import shutil
-import subprocess
 import sys
 
 import numpy as np
@@ -16,21 +13,13 @@ import pytest
 import audiolazy_b200 as ab
 from audiolazy_b200 import _build
 from conftest import GOLDEN
+from native_libs import check_every_kernel_is_launched, torch  # noqa: F401  (fixture)
 from zcross_emulation import block_sums, digest, zcross as emulate
 
 sys.path.insert(0, GOLDEN)
 from make_zcross import inputs  # noqa: E402
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def torch():
-  torch = pytest.importorskip("torch")
-  if not torch.cuda.is_available():
-    pytest.skip("no CUDA device")
-  torch.cuda.set_device(0)
-  return torch
 
 
 @pytest.fixture(scope="module")
@@ -211,17 +200,6 @@ def test_state_checks(torch):
   assert ab.Zcross(math.nan, 5).apply(x, state=nan.new_state(2)).shape == (2, 100)
 
 
-def _zcross_kernels():
-  cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-  filt = shutil.which("c++filt") or shutil.which("cu++filt") or "/usr/local/cuda/bin/cu++filt"
-  if not (os.path.exists(cuobjdump) and os.path.exists(filt)):
-    pytest.skip("cuobjdump / c++filt not available")
-  elf = subprocess.run([cuobjdump, "-elf", _build.ZCROSS_LIB_PATH], capture_output=True, text=True, check=True).stdout
-  mangled = sorted(set(re.findall(r"\.text\.(_Z\w+)", elf)))
-  names = subprocess.run([filt], input="\n".join(mangled), capture_output=True, text=True, check=True).stdout
-  return {n.split("(")[0].strip() for n in names.splitlines() if n.strip()}
-
-
 _LAUNCH_PROBE = r"""
 import sys
 sys.path.insert(0, sys.argv[1])
@@ -241,12 +219,4 @@ for name in sorted({e.name.split("(")[0].strip() for e in prof.events() if e.nam
 
 
 def test_every_zcross_kernel_is_launched(torch):
-  """The kernels the profiler sees launch are the kernels compiled into the library.  The profiling session runs in a
-  process of its own, so that it leaves no profiler state behind in this one."""
-  built = _zcross_kernels()
-  assert built, "no kernels found in %s" % _build.ZCROSS_LIB_PATH
-  root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-  run = subprocess.run([sys.executable, "-c", _LAUNCH_PROBE, root], capture_output=True, text=True, timeout=300)
-  assert run.returncode == 0, run.stderr[-2000:]
-  launched = {line.split(None, 1)[1] for line in run.stdout.splitlines() if line.startswith("LAUNCHED ")}
-  assert launched == built, (sorted(launched), sorted(built))
+  check_every_kernel_is_launched(_build.ZCROSS_LIB_PATH, _LAUNCH_PROBE)
