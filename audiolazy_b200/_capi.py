@@ -82,7 +82,7 @@ class NativeLib(object):
 class PlanInfo(ctypes.Structure):
   _fields_ = [(n, ctypes.c_int32) for n in
               ("abi_version", "kind", "n_channels", "n_sections", "num_taps", "monic", "state_doubles", "fp64_ops",
-               "device", "n_fp32_channels", "tier_tol_e9")] + [("reserved", ctypes.c_int32 * 5)]
+               "device", "n_fp32_channels", "tier_tol_e9", "time_parallel")] + [("reserved", ctypes.c_int32 * 4)]
 
 
 _i32, _i64, _f64, _vp, _p = ctypes.c_int32, ctypes.c_int64, ctypes.c_double, ctypes.c_void_p, ctypes.POINTER
@@ -180,6 +180,7 @@ class Plan(object):
     self.device = info.device
     self.n_fp32_channels = info.n_fp32_channels
     self.tier_tol = info.tier_tol_e9 * 1e-9
+    self.time_parallel = bool(info.time_parallel)   # few long streams may be evaluated time-parallel
     xd, yd = ctypes.c_int32(), ctypes.c_int32()
     _check(L.alz_plan_history(self._h, ctypes.byref(xd), ctypes.byref(yd)))
     self.xd, self.yd = xd.value, yd.value

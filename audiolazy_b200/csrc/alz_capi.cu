@@ -214,6 +214,65 @@ static int launch_generic(const alz_plan* p, AlzTileArgs ta, cudaStream_t st, co
 }
 
 static const int kBiquadKs[] = {1, 2, 3, 4, 6, 8};
+// a channel with a pole farther out than this is never put on the float32 tier, whatever its probe measures
+static const double kTierMaxRadius = 0.99;
+// The time-parallel evaluation adds a chunk's zero-state response F to the free response M s of its true initial
+// state.  When a numerator cancels (gammatone.sampled's head FIR at high rates: ~w^3 of its input) both are far larger
+// than the output, and their float64 rounding does not cancel.  A plan whose measured chunk error exceeds this is
+// always evaluated sequentially.  The error compounds over the chunks of a stream: over 10^6 samples the sampled
+// 192 kHz bank measured 9.6e-7 here and 3.9e-4 (400 times) against the oracle, so the limit keeps 400 times it
+// within the 1e-5 bar.  The 48 kHz sampled bank measures 2.1e-8 and stays within 3e-6 time-parallel.
+static const double kChunkMaxErr = 2.5e-8;
+static const long long kChunkProbeLen = 1024;          // about the chunk length the cost model picks for 10^6 samples
+
+// One chunk transition of one channel (sections (b, a), a[0] == 1) in plain float64 Direct Form I, on noise: the state
+// after 2L samples, F + M s as the time-parallel evaluation forms it, against the sequential state; both then filter the
+// next L samples.  Returns max |difference| / max |sequential output| over those samples.
+template <class Sec>
+static double chunk_error(const std::vector<Sec>& secs, long long L) {
+  const size_t K = secs.size();
+  struct Hist { std::vector<std::vector<double>> x, y; };
+  auto zero = [&]() {
+    Hist h;
+    for (const Sec& s : secs) { h.x.emplace_back(s.b.size() - 1, 0.0); h.y.emplace_back(s.a.size() - 1, 0.0); }
+    return h;
+  };
+  auto step = [&](Hist& h, double v) {
+    for (size_t k = 0; k < K; ++k) {
+      const Sec& s = secs[k];
+      std::vector<double>& xh = h.x[k];
+      std::vector<double>& yh = h.y[k];
+      double acc = s.b[0] * v;
+      for (size_t j = 1; j < s.b.size(); ++j) acc += s.b[j] * xh[j - 1];
+      for (size_t j = 1; j < s.a.size(); ++j) acc -= s.a[j] * yh[j - 1];
+      if (!xh.empty()) { std::copy_backward(xh.begin(), xh.end() - 1, xh.end()); xh[0] = v; }
+      if (!yh.empty()) { std::copy_backward(yh.begin(), yh.end() - 1, yh.end()); yh[0] = acc; }
+      v = acc;
+    }
+    return v;
+  };
+  std::vector<double> x(3 * L);
+  unsigned seed = 2024u;
+  for (auto& v : x) { seed = seed * 1664525u + 1013904223u; v = (double)(float)((double)(seed >> 8) * (2.0 / 16777216.0) - 1.0); }
+  Hist seq = zero();
+  for (long long n = 0; n < L; ++n) step(seq, x[n]);
+  Hist chunk = seq;                                   // -> M s: the state's response to L zero samples
+  for (long long n = 0; n < L; ++n) step(chunk, 0.0);
+  Hist f = zero();                                    // F: the second chunk from a zero state
+  for (long long n = L; n < 2 * L; ++n) { step(seq, x[n]); step(f, x[n]); }
+  for (size_t k = 0; k < K; ++k) {
+    for (size_t j = 0; j < chunk.x[k].size(); ++j) chunk.x[k][j] += f.x[k][j];
+    for (size_t j = 0; j < chunk.y[k].size(); ++j) chunk.y[k][j] += f.y[k][j];
+  }
+  double peak = 0.0, err = 0.0;
+  for (long long n = 2 * L; n < 3 * L; ++n) {
+    const double want = step(seq, x[n]), got = step(chunk, x[n]);
+    peak = std::max(peak, std::fabs(want));
+    const double d = std::fabs(got - want);
+    err = std::max(err, d == d ? d : 1e300);
+  }
+  return peak > 0.0 ? err / peak : (err > 0.0 ? 1e300 : 0.0);
+}
 
 // ----------------------------------------------------------------------------------
 extern "C" {
@@ -410,11 +469,20 @@ int32_t alz_plan_create_ex(const double* coef, const int32_t* desc, int32_t C, i
         r32[i] = (float)rec[i];
         if (rec[i] != 0.0 && !(std::fabs(rec[i]) > 1e-30 && std::fabs(rec[i]) < 1e30)) representable = false;
       }
+      // Near the unit circle float32 state rounding is amplified by ~1 / (1 - r), and on it (a pole cancelled by a zero,
+      // maverage.recursive(1)) the error random-walks with the length of the input, past any probe.
+      double radius = 0.0;
+      for (auto& s : secs[c]) {
+        const double a1 = s.a.size() > 1 ? s.a[1] : 0.0, a2 = s.a.size() > 2 ? s.a[2] : 0.0, disc = a1 * a1 - 4.0 * a2;
+        radius = std::max(radius, disc < 0.0 ? std::sqrt(a2) : 0.5 * (std::fabs(a1) + std::sqrt(disc)));
+      }
       if (tiering && representable) {
         p->tier_err[c] = probe_biquad(p, rec, tab32.data() + (size_t)c * stride);
-        if (p->tier_err[c] <= p->tier_tol) { p->tier[c] = 1; ++p->n_fp32; }
+        if (p->tier_err[c] <= p->tier_tol && radius <= kTierMaxRadius) { p->tier[c] = 1; ++p->n_fp32; }
       }
     }
+    if (!p->sequential)
+      for (int c = 0; c < C; ++c) p->chunk_err = std::max(p->chunk_err, chunk_error(secs[c], kChunkProbeLen));
     // ---- positions: interleave the tiers along blockIdx.x so both kinds of warp share every SM ----
     {
       std::vector<int> lst[2];
@@ -647,6 +715,7 @@ int32_t alz_plan_info_get(const alz_plan* p, alz_plan_info* out) {
   out->device = p->device;
   out->n_fp32_channels = p->n_fp32;
   out->tier_tol_e9 = (int32_t)std::min(2.0e9, p->tier_tol * 1e9 + 0.5);
+  out->time_parallel = p->kind == ALZ_KIND_BIQUAD && !p->sequential && p->chunk_err <= kChunkMaxErr;
   return ALZ_OK;
 }
 
@@ -826,7 +895,8 @@ static int apply_plain(const alz_plan* p, const float* x, float* y, double* stat
 // a warp's 32 virtual streams are chunks of ONE real stream: 3-D / 4-D tensor maps), L samples each.  `passes`: the
 // passes over all chunks the evaluation makes (2 for the bank, 3 for the bank with the envelope consumer).
 static bool chunk_geometry(const alz_plan* p, long long S, long long T, int passes, long long* P_out, long long* L_out) {
-  if (p->kind != ALZ_KIND_BIQUAD || p->sequential || env_int("ALZ_NO_TIME_PARALLEL", 0)) return false;
+  if (p->kind != ALZ_KIND_BIQUAD || p->sequential || p->chunk_err > kChunkMaxErr || env_int("ALZ_NO_TIME_PARALLEL", 0))
+    return false;
   if (T < std::max(2048, env_int("ALZ_TIME_PARALLEL_MIN", 16384)) || p->state_doubles > 32) return false;
   if (T >= (1ll << 31) || S > 65535) return false;
   const long long slots = (long long)p->sm_count * 24;

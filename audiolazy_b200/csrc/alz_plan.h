@@ -58,6 +58,7 @@ struct alz_plan {
   int tile_group = 2;          // TMA engine: tiles moved together by launches that fill the machine (1, 2, 4)
   bool parallel_sum = false;   // ALZ_PLAN_PARALLEL: plain float64 records, usable by alz_apply_sum_f32
   bool sequential = false;     // ALZ_PLAN_SEQUENTIAL: never evaluate time-parallel (bit-reproducible blocking)
+  double chunk_err = 0.0;      // biquad: measured error of one chunk transition of the time-parallel evaluation
   bool coef_small = false;     // kernel-parameter block size (kCoefSmall / kCoefLarge doubles)
   struct Chunk { void* block; int npos; };
   std::vector<Chunk> chunks;   // biquad: pre-built AlzBiquadArgs<NCOEF> blocks, <= NCOEF / stride positions each

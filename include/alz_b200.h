@@ -76,7 +76,9 @@ typedef struct alz_plan_info {
   int32_t device;            /* CUDA device ordinal the plan lives on                 */
   int32_t n_fp32_channels;   /* channels whose recurrence runs on the float32 tier (see alz_plan_tiers) */
   int32_t tier_tol_e9;       /* the tier decision's error threshold, in units of 1e-9 */
-  int32_t reserved[5];
+  int32_t time_parallel;     /* 1: a call on few long streams may be evaluated time-parallel (biquad kind, its
+                                measured chunk error within the bar, not ALZ_PLAN_SEQUENTIAL)                  */
+  int32_t reserved[4];
 } alz_plan_info;
 
 /* Thread-local description of the last error returned on this thread. */

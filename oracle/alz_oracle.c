@@ -31,7 +31,7 @@
 #include <stdlib.h>
 #include <string.h>
 
-#define ORC_MAX_TAPS 4096
+#define ORC_MAX_TAPS 8192
 
 /* One DF-I section over n samples, in place on a float64 buffer.
  * xh[j] = d_{j+1}, yh[j] = m_{j+1} on entry (histories), updated on exit. */

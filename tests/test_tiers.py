@@ -60,6 +60,8 @@ def test_tier_probe_matches_an_independent_emulation(designs):
   assert plan.kind == _capi.KIND_BIQUAD and plan.device == -1
   tier, probe = plan.tiers()
   assert plan.n_fp32_channels == int(tier.sum()) > 0
+  # probe > tol on every float64 channel holds here because no slaney channel has a pole beyond radius 0.99; elsewhere
+  # such a channel stays on float64 whatever it measures (tests/test_design_space.py)
   assert np.all(probe[tier == 1] <= plan.tier_tol) and np.all(probe[tier == 0] > plan.tier_tol)
   x = lcg_noise(8192)
   y64 = monic_emulation(bank, x, np.float64).astype(np.float64)
