@@ -327,7 +327,9 @@ def filter_stream_tv(num_terms, den_terms, seq, memory_init, zero):
   delay 0); ``coeff`` is a number or an iterator advanced once per input sample. A Stream a0
   becomes a variable gain exactly as the reference rewrites it: ``inv = 1 / a0`` and every
   other coefficient is multiplied by ``inv``. The per-sample coefficient values of a block
-  are evaluated on the host (they are the USER's streams) and uploaded with the block."""
+  are evaluated on the host (they are the USER's streams) and uploaded with the block.
+  When a coefficient Stream ends before the input, the Stream yields the samples before that
+  point and then raises ``RuntimeError``, as the reference does."""
   torch = torch_mod()
   device = torch.device("cuda", torch.cuda.current_device())
   _capi.set_device(device.index)
@@ -363,9 +365,9 @@ def filter_stream_tv(num_terms, den_terms, seq, memory_init, zero):
       cols = [pull(src, n) for _, src in sources]
       a0_vals = pull(a0, n)
       lens = [len(c) for c in cols if c is not None] + ([len(a0_vals)] if a0_vals is not None else [])
-      m = min([n] + lens)           # the shortest coefficient stream ends the output (zip semantics)
+      m = min([n] + lens)           # samples before the shortest coefficient stream ends
       if m == 0:
-        return
+        raise _coefficients_ended()
       inv = None if a0_vals is None else 1.0 / np.asarray(a0_vals[:m], dtype=np.float64)
       coef = np.empty((len(sources), m), dtype=np.float64)
       for row, (col, (is_den, src)) in enumerate(zip(cols, sources)):
@@ -378,6 +380,12 @@ def filter_stream_tv(num_terms, den_terms, seq, memory_init, zero):
       plan.apply_tv(x_dev.data_ptr(), y_dev.data_ptr(), state.data_ptr(), 1, m, m, m, c_dev.data_ptr(), m, cur())
       yield y_dev.cpu().numpy().tolist()
       if m < n:
-        return
+        raise _coefficients_ended()
 
   return Stream(it.chain.from_iterable(gen()))
+
+
+def _coefficients_ended():
+  """What the reference raises at the first input sample after a coefficient Stream ends: its generated filter loop
+  calls ``next()`` on the Stream, and Python turns a StopIteration leaving a generator into RuntimeError (PEP 479)."""
+  return RuntimeError("generator raised StopIteration")

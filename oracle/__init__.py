@@ -15,6 +15,9 @@ Two restatements of the reference's evaluator (``LinearFilter.__call__``, refere
 
 Both are pinned against golden vectors produced by the reference itself
 (``tests/golden/make_golden.py``) in ``tests/test_oracle.py``.
+
+:func:`tv_apply` states the time-varying contract of ``alz_apply_tv_f32`` (per-sample coefficient tables) in numpy;
+``tests/test_time_varying.py`` pins it to the reference's outputs (``tests/golden/make_tv.py``).
 """
 from __future__ import annotations
 
@@ -116,6 +119,50 @@ def bank_apply_f32(x, bank, threads: int = 1, out=None):
       raise RuntimeError("oracle failed")
 
   _threaded(run, S, threads)
+  return y
+
+
+def tv_apply(x, sections, table, xinit=None, yinit=None):
+  """The time-varying contract of ``alz_apply_tv_f32`` in float64, vectorised over streams.
+
+  ``x``: float32 rows ``[S][T]``.  ``sections``: the cascade, one list of ``(delay, is_den)`` taps per section, in
+  the order ``alz_plan_taps`` lists them (section by section, numerator then feedback taps, ascending delay).
+  ``table[i][n]``: the coefficient of tap ``i`` (counted over all sections) at sample ``n`` (``b_k / a_0`` for a
+  numerator tap, ``-a_k / a_0`` for a feedback tap); every stream uses the same table.  ``xinit`` / ``yinit``:
+  ``[K][h]`` initial input / output histories of each section as ``alz_state_init`` takes them (entry ``j`` is delay
+  ``j + 1``), or None for zeros.  Each product is rounded, then added to the sum in table order, starting from 0.0.
+  Returns ``y[S][T]`` float64, the last section's output."""
+  x = np.atleast_2d(np.asarray(x, dtype=np.float32)).astype(np.float64)
+  S, T = x.shape
+  table = np.asarray(table, dtype=np.float64)
+
+  def seeds(init, k, depth):
+    row = [] if init is None else [float(v) for v in np.asarray(init, dtype=np.float64)[k]]
+    row = (row + [0.0] * depth)[:depth]
+    return [np.full(S, v) for v in row]          # hist[d - 1] = the value at delay d
+
+  rows, xh, yh, first = [], [], [], 0      # rows[k]: (table row, delay, is_den) of section k's taps
+  for k, taps in enumerate(sections):
+    rows.append([(first + i, int(d), bool(den)) for i, (d, den) in enumerate(taps)])
+    first += len(taps)
+    xh.append(seeds(xinit, k, max([d for d, den in taps if not den] + [0])))
+    yh.append(seeds(yinit, k, max([d for d, den in taps if den] + [0])))
+  y = np.empty((S, T), dtype=np.float64)
+  for n in range(T):
+    inp = x[:, n]
+    for k, taps in enumerate(rows):
+      acc = np.zeros(S)
+      for i, d, den in taps:
+        past = yh[k][d - 1] if den else (inp if d == 0 else xh[k][d - 1])
+        acc = acc + table[i, n] * past
+      if xh[k]:
+        xh[k].insert(0, inp)
+        xh[k].pop()
+      if yh[k]:
+        yh[k].insert(0, acc)
+        yh[k].pop()
+      inp = acc
+    y[:, n] = inp
   return y
 
 
