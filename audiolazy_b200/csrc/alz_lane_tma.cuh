@@ -52,13 +52,27 @@ __device__ __forceinline__ void alz_tma_store_2d(const CUtensorMap* map, int c0,
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%1, %2}], [%3];\n"
                ::"l"(reinterpret_cast<unsigned long long>(map)), "r"(c0), "r"(c1), "r"(src) : "memory");
 }
-__device__ __forceinline__ void alz_tma_load_3d(unsigned dst, const CUtensorMap* map, int c0, int c1, int c2, unsigned mbar) {
-  asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];\n"
-               ::"r"(dst), "l"(reinterpret_cast<unsigned long long>(map)), "r"(c0), "r"(c1), "r"(c2), "r"(mbar) : "memory");
+// L2 cache policies for the bank's tile traffic (createpolicy), handed to the TMA as .L2::cache_hint operands.
+__device__ __forceinline__ unsigned long long alz_l2_evict_first() {
+  unsigned long long pol;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;\n" : "=l"(pol));
+  return pol;
 }
-__device__ __forceinline__ void alz_tma_store_4d(const CUtensorMap* map, int c0, int c1, int c2, int c3, unsigned src) {
-  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%1, %2, %3, %4}], [%5];\n"
-               ::"l"(reinterpret_cast<unsigned long long>(map)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(src) : "memory");
+__device__ __forceinline__ unsigned long long alz_l2_evict_last() {
+  unsigned long long pol;
+  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;\n" : "=l"(pol));
+  return pol;
+}
+__device__ __forceinline__ void alz_tma_load_3d(unsigned dst, const CUtensorMap* map, int c0, int c1, int c2, unsigned mbar,
+                                                unsigned long long pol) {
+  asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
+               " [%0], [%1, {%2, %3, %4}], [%5], %6;\n"
+               ::"r"(dst), "l"(reinterpret_cast<unsigned long long>(map)), "r"(c0), "r"(c1), "r"(c2), "r"(mbar), "l"(pol) : "memory");
+}
+__device__ __forceinline__ void alz_tma_store_4d(const CUtensorMap* map, int c0, int c1, int c2, int c3, unsigned src,
+                                                 unsigned long long pol) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%1, %2, %3, %4}], [%5], %6;\n"
+               ::"l"(reinterpret_cast<unsigned long long>(map)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(src), "l"(pol) : "memory");
 }
 __device__ __forceinline__ void alz_bulk_commit() { asm volatile("cp.async.bulk.commit_group;\n" ::: "memory"); }
 __device__ __forceinline__ void alz_bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;\n" ::: "memory"); }
@@ -181,9 +195,15 @@ __device__ __forceinline__ void alz_run_warp_tma(const AlzTileArgs& a, const Cor
   // profiles/r01_microbench_hbm_write.txt).  The load of the next group is exposed to this warp; the
   // other resident warps hide it.
   const int lg = NG >= 4 ? 2 : (NG >= 2 ? 1 : 0);
+  // L2 policy: every channel's warp of this stream group reads the same input tiles, at times that drift apart, while
+  // the output stream (64 x the input bytes for a 64-channel bank) is never read again.  Output tiles are stored
+  // evict-first and input tiles loaded evict-last, so the L2 gives up output lines first and a late reader still finds
+  // its tile there instead of fetching it from HBM again (DESIGN.md section 3: measured on the H100).
+  unsigned long long st_pol = 0, ld_pol = 0;
+  if (lane == 0) { st_pol = alz_l2_evict_first(); ld_pol = alz_l2_evict_last(); }
   if (lane == 0 && NG == 1) {   // tile 0 in flight
     alz_mbar_expect_tx(mbar0, ALZ_TMA_TILE_BYTES);
-    alz_tma_load_3d(tile0, tmx, tb, ld1, ld2, mbar0);
+    alz_tma_load_3d(tile0, tmx, tb, ld1, ld2, mbar0, ld_pol);
   }
   for (int i = 0; i < ntiles; ++i) {
     const int j = NG == 1 ? (i & 1) : (i & (NG - 1));   // buffer of tile i
@@ -196,14 +216,14 @@ __device__ __forceinline__ void alz_run_warp_tma(const AlzTileArgs& a, const Cor
           // finished READING it (it was issued a whole barrier-wait ago, so this normally does not block).
           if (i >= 1) alz_bulk_wait_read0();
           alz_mbar_expect_tx(mbar0 + 8 * (j ^ 1), ALZ_TMA_TILE_BYTES);
-          alz_tma_load_3d(tile0 + (j ^ 1) * ALZ_TMA_TILE_BYTES, tmx, tb + t0 + ALZ_TT, ld1, ld2, mbar0 + 8 * (j ^ 1));
+          alz_tma_load_3d(tile0 + (j ^ 1) * ALZ_TMA_TILE_BYTES, tmx, tb + t0 + ALZ_TT, ld1, ld2, mbar0 + 8 * (j ^ 1), ld_pol);
         }
       } else if (j == 0) {
         if (i > 0) alz_bulk_wait_read0();
         const int n = ntiles - i < NG ? ntiles - i : NG;
         for (int jj = 0; jj < n; ++jj) {
           alz_mbar_expect_tx(mbar0 + 8 * jj, ALZ_TMA_TILE_BYTES);
-          alz_tma_load_3d(tile0 + jj * ALZ_TMA_TILE_BYTES, tmx, tb + t0 + jj * ALZ_TT, ld1, ld2, mbar0 + 8 * jj);
+          alz_tma_load_3d(tile0 + jj * ALZ_TMA_TILE_BYTES, tmx, tb + t0 + jj * ALZ_TT, ld1, ld2, mbar0 + 8 * jj, ld_pol);
         }
       }
     }
@@ -217,12 +237,12 @@ __device__ __forceinline__ void alz_run_warp_tma(const AlzTileArgs& a, const Cor
     const bool last = i + 1 == ntiles;
     if (lane == 0 && !(a.exp & 2) && !Post::active) {
       if (NG == 1) {
-        if (!(tail_by_lanes && last)) alz_tma_store_4d(tmy, tb + t0, st1, st2, st3, tile0 + j * ALZ_TMA_TILE_BYTES);   // ragged last tile: stored after the loop
+        if (!(tail_by_lanes && last)) alz_tma_store_4d(tmy, tb + t0, st1, st2, st3, tile0 + j * ALZ_TMA_TILE_BYTES, st_pol);   // ragged last tile: stored after the loop
         alz_bulk_commit();
       } else if (j == NG - 1 || last) {
         for (int jj = 0; jj <= j; ++jj)
           if (!(tail_by_lanes && last && jj == j))
-            alz_tma_store_4d(tmy, tb + t0 - (j - jj) * ALZ_TT, st1, st2, st3, tile0 + jj * ALZ_TMA_TILE_BYTES);
+            alz_tma_store_4d(tmy, tb + t0 - (j - jj) * ALZ_TT, st1, st2, st3, tile0 + jj * ALZ_TMA_TILE_BYTES, st_pol);
         alz_bulk_commit();
       }
     }
