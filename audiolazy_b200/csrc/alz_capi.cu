@@ -976,6 +976,12 @@ static int chunk_transition(const alz_plan* p, long long L, cudaStream_t st, con
   return rc;
 }
 
+// 16-byte output stores (st.v4) need every row start aligned: y, the row stride ys and the stream stride ysS.
+// The cp.async engine steps between the 32 rows of a warp by ysS.
+static int vec_out_ok(const float* y, long long ys, long long ysS) {
+  return (((uintptr_t)y & 15) == 0 && (ys & 3) == 0 && (ysS & 3) == 0) ? 1 : 0;
+}
+
 static int apply_chunked(const alz_plan* p, const float* x, float* y, double* state, long long sstride, long long S,
                          long long T, long long xs, long long ys, long long P, long long L, cudaStream_t st) {
   const int C = p->C, d = p->state_doubles;
@@ -991,7 +997,7 @@ static int apply_chunked(const alz_plan* p, const float* x, float* y, double* st
   AlzTileArgs ta{};
   ta.x = x; ta.y = y; ta.S = V; ta.T = L; ta.xs = xs; ta.ys = ys; ta.ysS = (long long)C * ys; ta.C = C; ta.Stot = V;
   ta.vec_in = (((uintptr_t)x & 15) == 0 && (xs & 3) == 0) ? 1 : 0;          // L is a multiple of 32: chunk starts keep the alignment
-  ta.vec_out = (((uintptr_t)y & 15) == 0 && (ys & 3) == 0) ? 1 : 0;
+  ta.vec_out = vec_out_ok(y, ys, ta.ysS);
   ta.vP = (int)P;
   if (rc == ALZ_OK) {
     ta.exp = 2;                                                                 // pass 1: zero-state chunks, only the final states matter
@@ -1021,7 +1027,7 @@ static int apply_impl(const alz_plan* p, const float* x, float* y, double* state
   ta.T = T; ta.xs = xs; ta.ys = ys; ta.ysS = ysS; ta.C = p->C;
   ta.Stot = sstride / p->C;
   ta.vec_in = (((uintptr_t)x & 15) == 0 && (xs & 3) == 0) ? 1 : 0;
-  ta.vec_out = (((uintptr_t)y & 15) == 0 && (ys & 3) == 0) ? 1 : 0;
+  ta.vec_out = vec_out_ok(y, ys, ysS);   // channel-major rows (ysS = T) are 16-byte aligned only when T is a multiple of 4
   const long long kMaxStreams = 65535ll * 32;   // gridDim.y limit
   for (long long s0 = 0; s0 < S; s0 += kMaxStreams) {
     ta.S = std::min(kMaxStreams, S - s0);

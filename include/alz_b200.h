@@ -192,7 +192,8 @@ int32_t alz_apply_f32(const alz_plan* plan, const float* x_dev, float* y_dev,
  * NVLink -- with y_dev offset to its first channel; y_stream_stride >= n_channels * y_stride.  It also
  * expresses the CHANNEL-MAJOR layout y[C][S][T]: y_stream_stride = T, y_stride = n_streams * T (then
  * y_stride >= n_streams * y_stream_stride): the 32 rows a warp stores are 64 KB apart instead of C * 64 KB.
- * The time-parallel evaluation of few long streams is not used on this entry.
+ * With y_stream_stride == n_channels * y_stride (the dense layout) this entry is alz_apply_f32, time-parallel
+ * evaluation of few long streams included; any other stream stride is evaluated sequentially.
  */
 int32_t alz_apply_f32_ex(const alz_plan* plan, const float* x_dev, float* y_dev, double* state_dev,
                          int64_t n_streams, int64_t n_samples, int64_t x_stride, int64_t y_stride,
