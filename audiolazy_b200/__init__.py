@@ -7,7 +7,7 @@ Same names as the reference (``from audiolazy import ...``) for everything on th
 the reference lacks (``FilterBank``, ``gammatone_bank``, ``erb_space``); ``amdf`` with its batched
 form ``AmdfBank`` (many streams x many lags) and the ``freq2lag`` / ``lag2freq`` converters; ``zcross`` with its
 batched form ``Zcross`` (flags or per-block counts of many streams); ``lpc_frames`` with its batched form ``LpcFrames``
-(``lpc.kautocor`` of every block of many streams).
+(``lpc.kautocor`` or ``lpc.kcovar`` of every block of many streams).
 
 The per-sample recurrences run in hand-written sm_90a CUDA kernels behind the C ABIs of
 ``include/alz_b200.h``, ``include/alz_b200_amdf.h``, ``include/alz_b200_zcross.h`` and ``include/alz_b200_lpc.h``; importing this package does not need a GPU, calling a filter does.

@@ -9,10 +9,12 @@ recursions here work on coefficient lists, not on filter algebra, so results agr
 reference to rounding (tests: 1e-9 relative), not bit for bit.
 
 Frame-wise analysis runs on the GPU (``include/alz_b200_lpc.h``): :class:`LpcFrames` evaluates
-``lpc.kautocor`` of every block of ``Stream(x).blocks(size, hop)`` of many streams, continued block
-by block through an :class:`LpcState`, and :func:`lpc_frames` is its lazy form.  Those follow the
-reference's arithmetic operation for operation (CPython 3.12's compensated ``sum()`` included), so
-they equal ``lpc.kautocor`` of the reference bit for bit.
+``lpc.kautocor`` or ``lpc.kcovar`` of every block of ``Stream(x).blocks(size, hop)`` of many
+streams, continued block by block through an :class:`LpcState`, and :func:`lpc_frames` is its lazy
+form.  Those follow the reference's arithmetic operation for operation (CPython 3.12's compensated
+``sum()`` and, for ``kcovar``, its ZFilter algebra included), so they equal the reference's
+``lpc.kautocor`` / ``lpc.kcovar`` bit for bit -- not the host strategies of this module, which agree
+with it only to rounding.
 """
 from __future__ import annotations
 
@@ -258,6 +260,9 @@ LIB = _capi.NativeLib(_build.LPC_LIB_PATH, "LPC", {
   "alz_lpc_scratch_bytes": (_i64, [_i64, _i64, _i32]),
   "alz_lpc_apply_f32": (_i32, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _i64, _i64, _i32, _i32, _i32, _i32, _vp,
                                _i64, _vp]),
+  "alz_lpc_covar_scratch_bytes": (_i64, [_i64, _i64, _i32]),
+  "alz_lpc_covar_apply_f32": (_i32, [_vp, _i64, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _i64, _i64, _i32, _i32, _i32, _i32,
+                                     _vp, _i64, _vp]),
 }, {_capi.ALZ_ERR_INVALID: ValueError})
 #: every function include/alz_b200_lpc.h declares
 SYMBOLS = LIB.symbols
@@ -274,6 +279,21 @@ def _int_arg(name, value, lo, hi):
 
 
 LpcResult = collections.namedtuple("LpcResult", ["coef", "error", "failed"])
+
+#: the strategies of :data:`lpc` the GPU evaluates; the others solve with ``numpy.linalg.pinv``, whose SVD no kernel
+#: can reproduce bit for bit
+GPU_METHODS = ("kautocor", "kcovar")
+
+
+def _method(name):
+  """The canonical name of the :data:`lpc` strategy ``name`` (any of its aliases), which must be one the GPU runs."""
+  if not isinstance(name, str):
+    raise TypeError("method must be a string, not %s" % type(name).__name__)
+  for canon in GPU_METHODS:
+    if name in lpc and lpc[name] is lpc[canon]:
+      return canon
+  names = sorted(n for n in lpc._names if any(lpc[n] is lpc[c] for c in GPU_METHODS))
+  raise ValueError("method %r is not evaluated on the GPU; the supported ones are %s" % (name, ", ".join(names)))
 
 
 class LpcState(object):
@@ -302,22 +322,33 @@ class LpcState(object):
 
 
 class LpcFrames(object):
-  """Linear prediction (autocorrelation method, Levinson-Durbin) of every frame of many streams: frame ``k`` is the
-  block ``[k hop, k hop + size)`` of ``Stream(x).blocks(size, hop)`` (``hop`` defaults to ``size``), times ``window``
-  when one is given (``size`` reals), and its result equals the reference's ``lpc.kautocor(block, order)`` bit for bit.
+  """Linear prediction of every frame of many streams: frame ``k`` is the block ``[k hop, k hop + size)`` of
+  ``Stream(x).blocks(size, hop)`` (``hop`` defaults to ``size``), times ``window`` when one is given (``size`` reals),
+  and its result equals the reference's ``lpc.<method>(block, order)`` bit for bit.  ``method`` is ``"kautocor"``
+  (autocorrelation method, Levinson-Durbin) or ``"kcovar"`` (covariance method, a Gram-Schmidt lattice on the lag
+  matrix; it needs ``1 <= order < size``), or any alias :data:`lpc` gives them (``"kacorr"``, ``"kcov"``, ...).
 
   * ``lp.apply(x, state=None, final=False)`` -> :class:`LpcResult` ``(coef [S, F, order + 1] float64, error [S, F]
     float64, failed [S, F] uint8)`` for a CUDA float32 ``x[S, T]``: the F frames this call completes, plus, with
     ``final=True``, the reference's padded last block when it emits one.  ``coef[..., 0]`` is 1 and coefficients the
-    reference drops as zero are 0.0; ``failed`` marks the frames where the reference raises :class:`ParCorError`
-    (their coef and error are NaN).
+    reference drops as zero are 0.0; ``failed`` marks the frames where the reference raises (their coef and error are
+    NaN): 1 for kautocor's :class:`ParCorError` and kcovar's ``ZeroDivisionError``, 2 for kcovar's
+    ``ValueError("Unstable filter")``.
   * ``lp.acorr(x, state=None, final=False)`` -> the lags ``[S, F, order + 1]`` float64 of the same frames.
+  * ``lp.lag_matrix(x, state=None, final=False)`` -> the reference's ``lag_matrix(block, order)`` ``[S, F, order + 1,
+    order + 1]`` float64 of the same frames (``order < size``), the statistics of the covariance methods.
   * ``lp.new_state(S)`` -> :class:`LpcState`, to continue streams block by block; blocks of any lengths give the same
     bits as one call."""
 
-  def __init__(self, order, size, hop=None, window=None):
+  def __init__(self, order, size, hop=None, window=None, method="kautocor"):
+    self.method = _method(method)
     self.order = _int_arg("order", order, 0, MAX_ORDER)
     self.size = _int_arg("size", size, 1, MAX_SIZE)
+    if self.method == "kcovar":
+      if self.order < 1:
+        raise ValueError("kcovar needs order >= 1 (the reference raises IndexError at order 0)")
+      if self.order >= self.size:
+        raise ValueError("Block length should be higher than order")
     self.hop = self.size if hop is None else _int_arg("hop", hop, 1, 2 ** 31 - 1)
     if window is None:
       self.window = None
@@ -334,7 +365,7 @@ class LpcFrames(object):
     self._windows = {}
 
   def _key(self):
-    return (self.order, self.size, self.hop, self.window)
+    return (self.order, self.size, self.hop, self.window, self.method)
 
   def new_state(self, n_streams):
     return LpcState(self, n_streams)
@@ -355,11 +386,11 @@ class LpcFrames(object):
   def _check_state(self, state, S, device):
     _engine.check_state(state, LpcState, "LpcFrames", S, device)
     if state.key != self._key():
-      raise ValueError("state belongs to an LpcFrames with another order, size, hop or window")
+      raise ValueError("state belongs to an LpcFrames with another order, size, hop or window, or another method")
     if state.ended:
       raise ValueError("state was ended by a call with final=True")
 
-  def _run(self, x, state, final, levinson):
+  def _run(self, x, state, final, solve, covar):
     torch = _engine.torch_mod()
     x, S, T, xs = _engine.stream_input(x)
     L = self.order + 1
@@ -370,41 +401,54 @@ class LpcFrames(object):
       F = self.n_frames(state.consumed, T, final)
       dev = x.device
       w = self._window(dev)
+      wp = None if w is None else w.data_ptr()
       stream = torch.cuda.current_stream(dev).cuda_stream
-      if levinson:
+      apply, scratch_bytes = ((lib().alz_lpc_covar_apply_f32, lib().alz_lpc_covar_scratch_bytes) if covar else
+                              (lib().alz_lpc_apply_f32, lib().alz_lpc_scratch_bytes))
+      if solve:
         coef = torch.empty((S, F, L), dtype=torch.float64, device=dev)
         err = torch.empty((S, F), dtype=torch.float64, device=dev)
         failed = torch.empty((S, F), dtype=torch.uint8, device=dev)
-        nbytes = _check(lib().alz_lpc_scratch_bytes(S, F, self.order))
+        nbytes = _check(scratch_bytes(S, F, self.order))
         scratch = torch.empty(max(8, nbytes), dtype=torch.uint8, device=dev)   # on this stream: torch's allocator orders reuse
-        _check(lib().alz_lpc_apply_f32(x.data_ptr(), xs, None if w is None else w.data_ptr(), None, coef.data_ptr(),
-                                       err.data_ptr(), failed.data_ptr(), F, state.tensor.data_ptr(), S, T, self.order,
-                                       self.size, self.hop, int(bool(final)), scratch.data_ptr(), nbytes, stream))
+        _check(apply(x.data_ptr(), xs, wp, None, coef.data_ptr(), err.data_ptr(), failed.data_ptr(), F,
+                     state.tensor.data_ptr(), S, T, self.order, self.size, self.hop, int(bool(final)), scratch.data_ptr(),
+                     nbytes, stream))
         out = LpcResult(coef, err, failed)
       else:
-        out = torch.empty((S, F, L), dtype=torch.float64, device=dev)
-        _check(lib().alz_lpc_apply_f32(x.data_ptr(), xs, None if w is None else w.data_ptr(), out.data_ptr(), None,
-                                       None, None, F, state.tensor.data_ptr(), S, T, self.order, self.size, self.hop,
-                                       int(bool(final)), None, 0, stream))
+        out = torch.empty((S, F, L, L) if covar else (S, F, L), dtype=torch.float64, device=dev)
+        _check(apply(x.data_ptr(), xs, wp, out.data_ptr(), None, None, None, F, state.tensor.data_ptr(), S, T,
+                     self.order, self.size, self.hop, int(bool(final)), None, 0, stream))
     state.consumed += T
     state.ended = bool(final)
     return out
 
   def apply(self, x, state=None, final=False):
-    """Coefficients, squared prediction errors and failure flags of every frame this call emits."""
-    return self._run(x, state, final, True)
+    """Coefficients, squared prediction errors and failure codes of every frame this call emits."""
+    return self._run(x, state, final, True, self.method == "kcovar")
 
   def acorr(self, x, state=None, final=False):
     """Autocorrelation lags 0 .. order of every frame this call emits."""
-    return self._run(x, state, final, False)
+    return self._run(x, state, final, False, False)
+
+  def lag_matrix(self, x, state=None, final=False):
+    """The covariance-method lag matrix of every frame this call emits: ``[S, F, order + 1, order + 1]`` float64,
+    cell ``[j][i] = sum(b[n - i] * b[n - j] for n in order .. size - 1)`` (symmetric)."""
+    if self.order >= self.size:
+      raise ValueError("Block length should be higher than order")
+    return self._run(x, state, final, False, True)
 
 
-def lpc_frames(seq, order, size, hop=None, window=None):
+def lpc_frames(seq, order, size, hop=None, window=None, method="kautocor"):
   """Lazy Stream of the analysis filters of every block of ``Stream(seq).blocks(size, hop)`` (times ``window``, when
-  given): element ``k`` is the reference's ``lpc.kautocor(block k, order)``, a FIR :class:`ZFilter` with the squared
-  prediction error in ``.error``, bit for bit.  Reaching a frame where the reference raises :class:`ParCorError`
-  raises it, after the frames before it."""
-  lp = LpcFrames(order, size, hop, window)
+  given): element ``k`` is the reference's ``lpc.<method>(block k, order)`` (``"kautocor"`` or ``"kcovar"``, or an
+  alias), a FIR :class:`ZFilter` with the squared prediction error in ``.error``, bit for bit.  Reaching a frame where
+  the reference raises raises the same, after the frames before it: :class:`ParCorError` for kautocor,
+  ``ZeroDivisionError("Can't find next coefficient")`` or ``ValueError("Unstable filter")`` for kcovar, and kcovar of
+  order 0 raises ``IndexError`` at the first frame."""
+  method = _method(method)
+  covar0 = method == "kcovar" and isinstance(order, Integral) and order == 0
+  lp = LpcFrames(order, size, hop, window, "kautocor" if covar0 else method)
   torch = _engine.torch_mod()
   state = lp.new_state(1)                          # no device: raises at call time
   device = state.device
@@ -412,8 +456,14 @@ def lpc_frames(seq, order, size, hop=None, window=None):
   def frames(res):
     coef, err, failed = (t[0].cpu().numpy() for t in res)
     for c, e, f in zip(coef, err, failed):
+      if covar0:
+        raise IndexError("list index out of range")
       if f:
-        raise ParCorError("Can't find next PARCOR coefficient")
+        if method == "kautocor":
+          raise ParCorError("Can't find next PARCOR coefficient")
+        if f == 1:
+          raise ZeroDivisionError("Can't find next coefficient")
+        raise ValueError("Unstable filter")
       filt = ZFilter([1] + c[1:].tolist())
       filt.error = float(e)
       yield filt
