@@ -676,6 +676,10 @@ void alz_plan_destroy(alz_plan* p) {
   int cur = 0;
   cudaGetDevice(&cur);
   cudaSetDevice(p->device);
+  // Launches on any stream may still read the tables freed below (the window and generic kernels read d_coef, d_sec,
+  // d_tap_delay and d_far_* from global memory, the scans the cached M): cudaFree only "may perform implicit
+  // synchronization", so wait for the device (its green contexts included) first.
+  cudaDeviceSynchronize();
   if (p->pipe.ready) {
     for (int i = 0; i < AlzHostPipe::NBUF; ++i) {
       if (p->pipe.stream[i]) { cudaStreamSynchronize(p->pipe.stream[i]); cudaStreamDestroy(p->pipe.stream[i]); }
@@ -687,7 +691,7 @@ void alz_plan_destroy(alz_plan* p) {
     }
   }
   for (auto& ch : p->chunks) free(ch.block);
-  for (auto& e : p->m_cache) { cudaFree(e.M); cudaEventDestroy(e.ready); }
+  for (auto* e : p->m_cache) { cudaFree(e->M); cudaEventDestroy(e->ready); delete e; }
   free(p->win_block);
   cudaFree(p->d_far_delay);
   cudaFree(p->d_far_coef);
@@ -931,49 +935,94 @@ static bool chunk_geometry(const alz_plan* p, long long S, long long T, int pass
   return true;
 }
 
-// M = A^L (the chunk transition matrices, d x d per channel) on the device, ordered before the next work on `st`.  It
-// depends on the plan and the chunk length only: computed once per (plan, L), kept in the plan.
-static int chunk_transition(const alz_plan* p, long long L, cudaStream_t st, const double** M_out) {
-  const int C = p->C, d = p->state_doubles;
-  double* M = nullptr;
-  float *xz = nullptr, *ydum = nullptr;
-  int rc = ALZ_OK;
+// Frees a chunk-transition entry nobody holds.  Scans that read its M may still be queued on any stream (of any host
+// thread, or of a green context): cudaFree promises no ordering for memory from cudaMalloc ("may perform implicit
+// synchronization"), so the device is synchronised first (cudaDeviceSynchronize == cuCtxSynchronize on the primary
+// context, which also waits for the green contexts created from it).
+static void chunk_entry_free(alz_plan::MEntry* e) {
+  cudaDeviceSynchronize();
+  cudaFree(e->M);
+  cudaEventDestroy(e->ready);
+  cudaGetLastError();
+  delete e;
+}
+
+// Ends a call's use of an entry of chunk_transition, once every launch that reads its M is queued.
+static void chunk_release(const alz_plan* p, alz_plan::MEntry* e) {
   alz_plan* pm = const_cast<alz_plan*>(p);
-  cudaEvent_t m_ready = nullptr;
+  bool last;
   {
     std::lock_guard<std::mutex> lock(pm->m_mu);
-    for (auto& e : pm->m_cache)
-      if (e.L == L) { M = e.M; m_ready = e.ready; }
+    last = --e->users == 0 && e->evicted;
   }
-  if (M) {
-    ALZ_CUDA(cudaStreamWaitEvent(st, m_ready, 0));
-  } else {   // basis run: L zero samples from each unit state -> M = A^L, per channel (it does not depend on the stream)
-    ALZ_CUDA(cudaMalloc((void**)&M, (size_t)d * d * C * 8));
-    ALZ_CUDA(cudaMallocAsync((void**)&xz, (size_t)d * L * 4, st));
-    ALZ_CUDA(cudaMallocAsync((void**)&ydum, (size_t)d * C * L * 4, st));
-    ALZ_CUDA(cudaMemsetAsync(xz, 0, (size_t)d * L * 4, st));
-    const long long n = (long long)d * d * C;
-    alz_unit_state_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(M, d, C);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    AlzTileArgs tb{};
-    tb.x = xz; tb.y = ydum; tb.S = d; tb.T = L; tb.xs = L; tb.ys = L; tb.ysS = (long long)C * L; tb.C = C; tb.Stot = d;
-    tb.vec_in = tb.vec_out = 1;
-    tb.exp = 2;                                                                 // its outputs are not needed: no tile stores
-    rc = apply_launch(p, tb, M, (long long)d * C, st, nullptr, 0);
-    cudaFreeAsync(xz, st); cudaFreeAsync(ydum, st);
-    ALZ_CUDA(cudaEventCreateWithFlags(&m_ready, cudaEventDisableTiming));
-    ALZ_CUDA(cudaEventRecord(m_ready, st));
+  if (last) chunk_entry_free(e);
+}
+
+// M = A^L (the chunk transition matrices, d x d per channel) on the device, ordered before the next work on `st`.  It
+// depends on the plan and the chunk length only: computed once per (plan, L), kept in the plan.  The entry is held
+// for the caller, which hands it back with chunk_release after queuing its scan; until then no other call (thread)
+// frees it.  The basis run is queued under the lock, so that calls that miss the same L at once compute it once.
+static int chunk_transition(const alz_plan* p, long long L, cudaStream_t st, alz_plan::MEntry** out) {
+  const int C = p->C, d = p->state_doubles;
+  alz_plan* pm = const_cast<alz_plan*>(p);
+  alz_plan::MEntry* e = nullptr;
+  alz_plan::MEntry* victim = nullptr;
+  *out = nullptr;
+  {
     std::lock_guard<std::mutex> lock(pm->m_mu);
-    if (pm->m_cache.size() >= 8) {                 // bounded: drop the oldest entry (its users were ordered before this point on their streams)
-      cudaStreamSynchronize(st);
-      cudaFree(pm->m_cache.front().M);
-      cudaEventDestroy(pm->m_cache.front().ready);
-      pm->m_cache.erase(pm->m_cache.begin());
+    for (auto* c : pm->m_cache)
+      if (c->L == L) e = c;
+    if (e) {
+      ++e->users;
+    } else {   // basis run: L zero samples from each unit state -> M = A^L, per channel (it does not depend on the stream)
+      double* M = nullptr;
+      float *xz = nullptr, *ydum = nullptr;
+      cudaEvent_t ready = nullptr;
+      ALZ_CUDA(cudaMalloc((void**)&M, (size_t)d * d * C * 8));
+      cudaError_t ce = cudaEventCreateWithFlags(&ready, cudaEventDisableTiming);
+      if (ce == cudaSuccess) ce = cudaMallocAsync((void**)&xz, (size_t)d * L * 4, st);
+      if (ce == cudaSuccess) ce = cudaMallocAsync((void**)&ydum, (size_t)d * C * L * 4, st);
+      if (ce == cudaSuccess) ce = cudaMemsetAsync(xz, 0, (size_t)d * L * 4, st);
+      int rc = ALZ_OK;
+      if (ce == cudaSuccess) {
+        const long long n = (long long)d * d * C;
+        alz_unit_state_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(M, d, C);
+        g_launches.fetch_add(1, std::memory_order_relaxed);
+        AlzTileArgs tb{};
+        tb.x = xz; tb.y = ydum; tb.S = d; tb.T = L; tb.xs = L; tb.ys = L; tb.ysS = (long long)C * L; tb.C = C; tb.Stot = d;
+        tb.vec_in = tb.vec_out = 1;
+        tb.exp = 2;                                                             // its outputs are not needed: no tile stores
+        rc = apply_launch(p, tb, M, (long long)d * C, st, nullptr, 0);
+      }
+      if (xz) cudaFreeAsync(xz, st);
+      if (ydum) cudaFreeAsync(ydum, st);
+      if (ce == cudaSuccess && rc == ALZ_OK) ce = cudaEventRecord(ready, st);
+      if (ce != cudaSuccess || rc != ALZ_OK) {
+        cudaStreamSynchronize(st);                 // the basis run may be queued: M stays allocated until it is done
+        cudaFree(M);
+        if (ready) cudaEventDestroy(ready);
+        cudaGetLastError();
+        return rc != ALZ_OK ? rc : fail(ALZ_ERR_CUDA, "chunk transition: %s", cudaGetErrorString(ce));
+      }
+      e = new alz_plan::MEntry{L, M, ready, 1, false};
+      if (pm->m_cache.size() >= 8) {               // bounded: drop the oldest entry; calls that still hold it free it
+        victim = pm->m_cache.front();
+        pm->m_cache.erase(pm->m_cache.begin());
+        victim->evicted = true;
+        if (victim->users > 0) victim = nullptr;
+      }
+      pm->m_cache.push_back(e);
     }
-    pm->m_cache.push_back({L, M, m_ready});
   }
-  *M_out = M;
-  return rc;
+  if (victim) chunk_entry_free(victim);
+  // held: nobody destroys e->ready before this wait is queued (for the call that computed M it orders nothing)
+  const cudaError_t we = cudaStreamWaitEvent(st, e->ready, 0);
+  if (we != cudaSuccess) {
+    chunk_release(p, e);
+    return fail(ALZ_ERR_CUDA, "cudaStreamWaitEvent failed: %s", cudaGetErrorString(we));
+  }
+  *out = e;
+  return ALZ_OK;
 }
 
 // 16-byte output stores (st.v4) need every row start aligned: y, the row stride ys and the stream stride ysS.
@@ -989,11 +1038,11 @@ static int apply_chunked(const alz_plan* p, const float* x, float* y, double* st
   const size_t nstate = (size_t)d * V * C;
   keep_async_pool();
   double *Z1 = nullptr, *Z2 = nullptr;
-  const double* M = nullptr;
+  alz_plan::MEntry* m = nullptr;
   ALZ_CUDA(cudaMallocAsync((void**)&Z1, nstate * 8, st));
   ALZ_CUDA(cudaMallocAsync((void**)&Z2, nstate * 8, st));
   ALZ_CUDA(cudaMemsetAsync(Z1, 0, nstate * 8, st));
-  int rc = chunk_transition(p, L, st, &M);
+  int rc = chunk_transition(p, L, st, &m);
   AlzTileArgs ta{};
   ta.x = x; ta.y = y; ta.S = V; ta.T = L; ta.xs = xs; ta.ys = ys; ta.ysS = (long long)C * ys; ta.C = C; ta.Stot = V;
   ta.vec_in = (((uintptr_t)x & 15) == 0 && (xs & 3) == 0) ? 1 : 0;          // L is a multiple of 32: chunk starts keep the alignment
@@ -1004,8 +1053,12 @@ static int apply_chunked(const alz_plan* p, const float* x, float* y, double* st
     rc = apply_launch(p, ta, Z1, V * C, st, nullptr, 0);
   }
   if (rc == ALZ_OK) {
-    alz_chunk_scan_kernel<<<dim3((unsigned)C, (unsigned)S), 32, 0, st>>>(Z1, Z2, M, state, sstride, sstride / C, d, C, S, P);
-    ALZ_CUDA(cudaGetLastError());
+    alz_chunk_scan_kernel<<<dim3((unsigned)C, (unsigned)S), 32, 0, st>>>(Z1, Z2, m->M, state, sstride, sstride / C, d, C, S, P);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) rc = fail(ALZ_ERR_CUDA, "chunk scan launch failed: %s", cudaGetErrorString(e));
+  }
+  if (m) chunk_release(p, m);
+  if (rc == ALZ_OK) {
     g_launches.fetch_add(1, std::memory_order_relaxed);
     ta.exp = 0;
     rc = apply_launch(p, ta, Z2, V * C, st, nullptr, 0);                        // pass 2: every chunk from its true initial state
@@ -1104,7 +1157,7 @@ static int envelope_chunked(const alz_plan* p, const float* x, float* env, doubl
   const size_t nstate = (size_t)d * V * C, nenv = (size_t)V * C;
   keep_async_pool();
   double *Z1 = nullptr, *Z2 = nullptr, *E = nullptr, *E2 = nullptr, *RL = nullptr;
-  const double* M = nullptr;
+  alz_plan::MEntry* m = nullptr;
   ALZ_CUDA(cudaMallocAsync((void**)&Z1, nstate * 8, st));
   ALZ_CUDA(cudaMallocAsync((void**)&Z2, nstate * 8, st));
   ALZ_CUDA(cudaMallocAsync((void**)&E, nenv * 8, st));
@@ -1116,7 +1169,7 @@ static int envelope_chunked(const alz_plan* p, const float* x, float* env, doubl
     const std::vector<double> rl((size_t)C, std::pow(ep.R, (double)L));
     ALZ_CUDA(cudaMemcpyAsync(RL, rl.data(), (size_t)C * 8, cudaMemcpyHostToDevice, st));
   }
-  int rc = chunk_transition(p, L, st, &M);
+  int rc = chunk_transition(p, L, st, &m);
   AlzTileArgs ta{};
   // y feeds only the (unused) output tensor map: x stands in, as in the sequential launch
   ta.x = x; ta.y = const_cast<float*>(x); ta.S = V; ta.T = L; ta.xs = xs; ta.ys = xs; ta.ysS = (long long)C * xs; ta.C = C;
@@ -1129,8 +1182,12 @@ static int envelope_chunked(const alz_plan* p, const float* x, float* env, doubl
     ta.exp = 0;
   }
   if (rc == ALZ_OK) {
-    alz_chunk_scan_kernel<<<dim3((unsigned)C, (unsigned)S), 32, 0, st>>>(Z1, Z2, M, state, sstride, sstride / C, d, C, S, P);
-    ALZ_CUDA(cudaGetLastError());
+    alz_chunk_scan_kernel<<<dim3((unsigned)C, (unsigned)S), 32, 0, st>>>(Z1, Z2, m->M, state, sstride, sstride / C, d, C, S, P);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) rc = fail(ALZ_ERR_CUDA, "chunk scan launch failed: %s", cudaGetErrorString(e));
+  }
+  if (m) chunk_release(p, m);
+  if (rc == ALZ_OK) {
     g_launches.fetch_add(1, std::memory_order_relaxed);
     ALZ_CUDA(cudaMemcpyAsync(Z1, Z2, nstate * 8, cudaMemcpyDeviceToDevice, st));   // pass 2 overwrites Z2; pass 3 needs it
     ta.state = Z2; ta.sstride = V * C;

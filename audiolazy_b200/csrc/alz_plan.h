@@ -91,9 +91,12 @@ struct alz_plan {
   double* d_fr_coef = nullptr;
   int fr_K = 0;
   int* d_fr_desc = nullptr;
-  struct MEntry { long long L; double* M; cudaEvent_t ready; };
-  std::mutex m_mu;               // guards m_cache (NOT host_mu: alz_apply_f32_host holds that one across its launches)
-  std::vector<MEntry> m_cache;   // time-parallel evaluation: chunk transition matrices A^L per chunk length (device)
+  // users: calls that hold the entry between their lookup and the launch of their last reader of M (chunk_release);
+  // an entry evicted while held is freed by the call that drops its last user
+  struct MEntry { long long L; double* M; cudaEvent_t ready; int users; bool evicted; };
+  std::mutex m_mu;                // guards m_cache and every entry's users / evicted (NOT host_mu: alz_apply_f32_host
+                                  // holds that one across its launches)
+  std::vector<MEntry*> m_cache;   // time-parallel evaluation: chunk transition matrices A^L per chunk length (device)
   std::mutex host_mu;
   AlzHostPipe pipe;
 };

@@ -327,7 +327,13 @@ int32_t alz_amdf_plan_create(const int32_t* n_taps, const int32_t* delays, const
 void alz_amdf_plan_destroy(void* plan) {
   auto p = static_cast<AmdfPlan*>(plan);
   if (!p) return;
+  // launches queued on any stream may still read the lag table: cudaFree only "may perform implicit synchronization"
+  int cur = -1;
+  cudaGetDevice(&cur);
+  cudaSetDevice(p->device);
+  cudaDeviceSynchronize();
   cudaFree(p->d_lags);
+  if (cur >= 0) cudaSetDevice(cur);
   cudaGetLastError();
   delete p;
 }
