@@ -224,6 +224,7 @@ static const double kTierMaxRadius = 0.99;
 // within the 1e-5 bar.  The 48 kHz sampled bank measures 2.1e-8 and stays within 3e-6 time-parallel.
 static const double kChunkMaxErr = 2.5e-8;
 static const long long kChunkProbeLen = 1024;          // about the chunk length the cost model picks for 10^6 samples
+static const int kTileGroup4MaxFp64 = 16;               // most FP64 instructions per channel-sample for tile group 4
 
 // One chunk transition of one channel (sections (b, a), a[0] == 1) in plain float64 Direct Form I, on noise: the state
 // after 2L samples, F + M s as the time-parallel evaluation forms it, against the sequential state; both then filter the
@@ -518,8 +519,14 @@ int32_t alz_plan_create_ex(const double* coef, const int32_t* desc, int32_t C, i
       memcpy(blk + 2 * sizeof(int), p->h_tab.data() + (size_t)p0 * stride, (size_t)npos * stride * sizeof(double));
       p->chunks.push_back({blk, npos});
     }
-    p->tile_group = env_int("ALZ_TILE_GROUP", 2);
-    if (p->tile_group != 1 && p->tile_group != 2 && p->tile_group != 4) p->tile_group = 2;
+    // Tile group of the launches that fill the machine: 4 (512 B pieces of every output row, 13 CTAs per SM on an H100)
+    // when the arithmetic hides under the output stores; a plan with more FP64 work per channel-sample is bound by
+    // issue and keeps 2, whose 24 CTAs per SM hide more of it.  Measured at the same shape (4096 x 16384,
+    // profiles/h100_tile_group4_ab.txt): klapuri (fp64_ops 10) and slaney (12) gain 3 % with 4, the head-FIR sampled
+    // bank (19) loses 5 %; the bound lies between them.
+    const int group = env_int("ALZ_TILE_GROUP", 0);
+    p->tile_group_forced = group == 1 || group == 2 || group == 4;
+    p->tile_group = p->tile_group_forced ? group : (p->fp64_ops <= kTileGroup4MaxFp64 ? 4 : 2);
   } else if (Kmax == 1 && !(flags & ALZ_PLAN_FORCE_GENERIC) && C * 32 <= kCoefLarge && !env_int("ALZ_NO_WINDOW", 0)) {
     // ---- window: one section per channel, dense near taps in registers + prefetched far taps (alz_window.cuh) ----
     p->kind = ALZ_KIND_GENERIC;

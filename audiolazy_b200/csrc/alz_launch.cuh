@@ -14,7 +14,8 @@
 // parameters; two sizes so that small filters do not push 28 KB per launch.
 static const int kCoefSmall = 512, kCoefLarge = 3584;
 static const int kWarpsPerSm = 22;      // cp.async engine: 2 x 4608 B tile buffers + 1 KB CTA reserve -> 22 CTAs per SM
-static const int kWarpsPerSmTma = 24;   // TMA engine: 2 x 4096 B + barriers + reserve -> 24 CTAs per SM
+static const int kWarpsPerSmTma = 24;   // TMA engine launch bounds: 80 registers, 24 CTAs per SM (bank launches query it)
+static const double kSegTailIdle = 0.02;   // largest share of a bank launch's warp slots its last wave may leave idle
 
 // Both precision tiers live in one kernel: the tier of a grid position is warp (= CTA) uniform,
 // read from the position's coefficient record.  Float64 and float32 warps of different channels
@@ -72,6 +73,23 @@ static int launch_envelope_t(const alz_plan* p, AlzTileArgs ta, cudaStream_t st)
   return ALZI_OK;
 }
 
+// CTAs of the TMA bank kernel `kern` resident per SM with the tile buffers of group size `ng`: the occupancy of the
+// instantiation on the plan's device (registers, shared memory, the 1 KB reserve per CTA), queried once per plan and
+// buffer count.  The shared-memory carveout is asked for at its maximum, so that on an H100 13 CTAs of 4 tiles (17.4 KB
+// each with the reserve) share the 228 KB of an SM.
+static int tma_ctas_per_sm(const alz_plan* p, const void* kern, int ng, long long* out) {
+  std::atomic<int>& cached = p->tma_ctas_per_sm[ng >= 4 ? 1 : 0];
+  int n = cached.load(std::memory_order_relaxed);
+  if (n == 0) {
+    ALZ_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    ALZ_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, 32, ALZ_TMA_SMEM_FOR(ng)));
+    if (n < 1) return alzi_fail(ALZI_ERR_UNSUPPORTED, "bank kernel: no CTA of %d tiles fits on an SM", ng < 2 ? 2 : ng);
+    cached.store(n, std::memory_order_relaxed);
+  }
+  *out = n;
+  return ALZI_OK;
+}
+
 // One launch: positions [p0, p0+npos) x stream groups of `ta` (ta.S <= 65535*32 streams).  `block` is
 // the plan's pre-built AlzBiquadArgs<NCOEF> for this chunk.
 template <int K, int NB, int MONIC, int NCOEF, int NB0, int ZMASK>
@@ -79,43 +97,67 @@ static int launch_biquad_chunk(const alz_plan* p, AlzTileArgs ta, const void* bl
   const long long groups = (ta.S + 31) / 32;
   CUtensorMap tmx, tmy;
   if (alzi_make_tensor_maps(ta, &tmx, &tmy)) {
-    // A launch of only a few waves of warps loses its last, partly filled wave: cut time into
-    // segments chained through the state (alz_lane_tma.cuh) so the next segment fills the tail.
+    const void* kern = (const void*)alz_biquad_tma_kernel<K, NB, MONIC, NCOEF, NB0, ZMASK>;
     const long long warps = (long long)npos * groups;
-    int ng = warps >= (long long)p->sm_count * kWarpsPerSmTma ? p->tile_group : 1;
+    const long long min_len = std::max(32, alzi_env_int("ALZ_SEG_MIN", 1024));
+    const bool can_segment = ta.vP == 0 && ta.T >= 2 * min_len && !alzi_env_int("ALZ_NO_SEGMENT", 0);
+    // Tile group: the plan's (alz_capi.cu) when the launch fills the machine at that group's occupancy.  A launch that
+    // fits in one wave of the one-tile pipeline and cannot be cut into time segments stays there: with 4 tiles (13 CTAs
+    // per SM instead of 24 on an H100) it would run a second, mostly idle wave.
+    long long per_one = 0, per_group = 0;
+    int rc = tma_ctas_per_sm(p, kern, 1, &per_one);
+    if (rc == ALZI_OK) rc = tma_ctas_per_sm(p, kern, p->tile_group, &per_group);
+    if (rc != ALZI_OK) return rc;
+    const bool fills = warps >= p->sm_count * per_group && (can_segment || warps >= p->sm_count * per_one);
+    int ng = p->tile_group_forced || fills ? p->tile_group : 1;
     ng = alzi_env_int("ALZ_TMA_PAIRED", ng);     // 0/1 = prefetch pipeline, 2 / 4 = tile groups
     if (ng != 2 && ng != 4) ng = 1;
     ta.paired = ng;
     ta.exp |= alzi_env_int("ALZ_EXP", 0);
     const size_t smem = ALZ_TMA_SMEM_FOR(ng);
-    const long long per_sm = std::min<long long>(kWarpsPerSmTma, (228 * 1024) / (long long)(smem + 1024));
+    long long per_sm = 0;
+    if ((rc = tma_ctas_per_sm(p, kern, ng, &per_sm)) != ALZI_OK) return rc;
     const long long slots = (long long)p->sm_count * per_sm;
-    long long nseg = 1;
-    if (ta.vP == 0 && warps > slots && warps < 8 * slots && ta.T >= 2048 && !alzi_env_int("ALZ_NO_SEGMENT", 0)) {
-      const long long waves = std::max(1, alzi_env_int("ALZ_SEG_WAVES", 16)), min_len = std::max(32, alzi_env_int("ALZ_SEG_MIN", 1024));
-      nseg = std::min((waves * slots + warps - 1) / warps, ta.T / min_len);
-      const long long quantum = 32ll * ng;     // whole tile groups per segment
-      const long long len = ((ta.T + nseg - 1) / nseg + quantum - 1) / quantum * quantum;
-      nseg = (ta.T + len - 1) / len;
-      if (nseg > 1 && groups * nseg <= 65535) {
-        const size_t words = (size_t)npos + (size_t)npos * groups;
-        unsigned* sync = nullptr;
-        alzi_keep_async_pool();
-        ALZ_CUDA(cudaMallocAsync(&sync, words * 4, st));
-        if (cudaMemsetAsync(sync, 0, words * 4, st) != cudaSuccess) {
-          cudaFreeAsync(sync, st);
-          ALZ_CUDA(cudaGetLastError());
-        }
-        ta.nseg = (int)nseg; ta.seg_len = len; ta.sync = sync;
-      } else {
-        nseg = 1;
+    // Time segments chained through the state (alz_lane_tma.cuh).  The warps run in waves of `slots`, and a partly
+    // filled last wave idles the rest of the slots for a whole wave: a share ceil(n w / s) s - n w of ceil(n w / s) s
+    // when the launch is cut into n segments, n w warps of 1 / n the length.  A launch that would idle more than
+    // kSegTailIdle of its slots is cut into the fewest segments (whole tile groups, >= min_len samples) that stay
+    // within it, else into the count that idles least.  A count that idles no less than the whole launch is not taken:
+    // it would pay for the segment flags and the chained waits and gain nothing.
+    auto idle = [&](long long n) {
+      const long long cap = (n * warps + slots - 1) / slots * slots;
+      return (double)(cap - n * warps) / (double)cap;
+    };
+    long long nseg = 1, len = ta.T;
+    if (can_segment && warps > slots && idle(1) > kSegTailIdle) {
+      const long long quantum = 32ll * ng;
+      double best = idle(1);
+      for (long long n = 2; n <= ta.T / min_len && groups * n <= 65535; ++n) {
+        const long long ln = ((ta.T + n - 1) / n + quantum - 1) / quantum * quantum;
+        if ((ta.T + ln - 1) / ln != n) continue;   // fewer segments once rounded: that count is weighed on its own
+        const double f = idle(n);
+        if (f < best) { best = f; nseg = n; len = ln; }
+        if (f <= kSegTailIdle) break;
       }
     }
+    if (alzi_env_int("ALZ_LOG_LAUNCH", 0))
+      fprintf(stderr, "alz bank launch: %lld warps, tile group %d, %lld CTAs per SM (%lld slots), %lld segment(s) of %lld samples\n",
+              warps, ng, per_sm, slots, nseg, len);
+    if (nseg > 1) {
+      const size_t words = (size_t)npos + (size_t)npos * groups;
+      unsigned* sync = nullptr;
+      alzi_keep_async_pool();
+      ALZ_CUDA(cudaMallocAsync(&sync, words * 4, st));
+      if (cudaMemsetAsync(sync, 0, words * 4, st) != cudaSuccess) {
+        cudaFreeAsync(sync, st);
+        ALZ_CUDA(cudaGetLastError());
+      }
+      ta.nseg = (int)nseg; ta.seg_len = len; ta.sync = sync;
+    }
     ta.groups = (int)groups;
-    auto kern = alz_biquad_tma_kernel<K, NB, MONIC, NCOEF, NB0, ZMASK>;
     if (smem > 48 * 1024) return alzi_fail(ALZI_ERR_UNSUPPORTED, "tile group too large");
     void* args[4] = {(void*)&ta, const_cast<void*>(block), (void*)&tmx, (void*)&tmy};
-    const cudaError_t e = cudaLaunchKernel((const void*)kern, dim3((unsigned)npos, (unsigned)(groups * nseg)), dim3(32), args, smem, st);
+    const cudaError_t e = cudaLaunchKernel(kern, dim3((unsigned)npos, (unsigned)(groups * nseg)), dim3(32), args, smem, st);
     if (ta.sync) cudaFreeAsync(ta.sync, st);
     ALZ_CUDA(e);
   } else {

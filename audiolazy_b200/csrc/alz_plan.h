@@ -55,7 +55,11 @@ struct alz_plan {
   int n_fp32 = 0;              // biquad: channels on the float32 tier
   double tier_tol = 0.0;       // measured-error threshold the tier decision used
   int probe_len = 8192;        // samples per probe signal of the tier decision
-  int tile_group = 2;          // TMA engine: tiles moved together by launches that fill the machine (1, 2, 4)
+  int tile_group = 4;          // TMA engine: tiles moved together by launches that fill the machine (1, 2, 4; alz_capi.cu)
+  bool tile_group_forced = false;   // ALZ_TILE_GROUP: tile_group on every TMA launch, whatever its size
+  // TMA bank kernel: CTAs resident per SM with 2 / 4 tile buffers (occupancy query on the plan's first TMA launch; 0 = not
+  // yet).  Host threads that race on the first launch store the same value.
+  mutable std::atomic<int> tma_ctas_per_sm[2] = {};
   bool parallel_sum = false;   // ALZ_PLAN_PARALLEL: plain float64 records, usable by alz_apply_sum_f32
   bool sequential = false;     // ALZ_PLAN_SEQUENTIAL: never evaluate time-parallel (bit-reproducible blocking)
   double chunk_err = 0.0;      // biquad: measured error of one chunk transition of the time-parallel evaluation
