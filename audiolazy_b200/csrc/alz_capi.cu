@@ -13,6 +13,7 @@
 #include <cmath>
 #include <cstring>
 #include <map>
+#include <memory>
 #include <thread>
 
 #include <sys/mman.h>
@@ -226,6 +227,8 @@ static const double kChunkMaxErr = 2.5e-8;
 static const long long kChunkProbeLen = 1024;          // about the chunk length the cost model picks for 10^6 samples
 static const int kTileGroup4MaxFp64 = 16;               // most FP64 instructions per channel-sample for tile group 4
 
+struct Sec { std::vector<double> b, a; };   // one section of a cascade; a[0] == 1 after normalisation (kept for indexing)
+
 // One chunk transition of one channel (sections (b, a), a[0] == 1) in plain float64 Direct Form I, on noise: the state
 // after 2L samples, F + M s as the time-parallel evaluation forms it, against the sequential state; both then filter the
 // next L samples.  Returns max |difference| / max |sequential output| over those samples.
@@ -275,6 +278,402 @@ static double chunk_error(const std::vector<Sec>& secs, long long L) {
   return peak > 0.0 ? err / peak : (err > 0.0 ? 1e300 : 0.0);
 }
 
+// Makes a plan's device current for the rest of the scope and gives the caller's device back on every return path.
+struct DeviceScope {
+  int prev = -1;
+  bool switched = false;
+  cudaError_t status;
+  explicit DeviceScope(int device) {
+    status = cudaGetDevice(&prev);
+    if (status == cudaSuccess && prev != device) {
+      status = cudaSetDevice(device);
+      switched = status == cudaSuccess;
+    }
+  }
+  ~DeviceScope() { if (switched) cudaSetDevice(prev); }
+};
+
+// Device scratch from the stream-ordered pool, freed on `st` when the scope ends (on every return path): after the
+// work already queued there, so the caller only has to make sure every other stream that uses it is done.
+template <class T>
+struct StreamScratch {
+  T* ptr = nullptr;
+  cudaStream_t st;
+  explicit StreamScratch(cudaStream_t s) : st(s) {}
+  ~StreamScratch() { if (ptr) cudaFreeAsync(ptr, st); }
+  StreamScratch(const StreamScratch&) = delete;
+  StreamScratch& operator=(const StreamScratch&) = delete;
+  cudaError_t alloc(size_t n) { return cudaMallocAsync((void**)&ptr, n * sizeof(T), st); }
+};
+// A buffer of cudaMalloc, freed when the scope ends.  The host entries size theirs by the whole batch: the pool, which
+// keeps what it is given back once the time-parallel evaluation has run, would hold on to it after the call.
+typedef std::unique_ptr<double, cudaError_t (*)(void*)> DeviceBuffer;
+
+// A plan's host table and the device pointer of the plan that receives its copy.
+struct Upload { void** dst; const void* src; size_t bytes; };
+template <class T>
+static Upload table(T** dst, const std::vector<T>& src) { return {(void**)dst, src.data(), src.size() * sizeof(T)}; }
+
+// Copies a plan's tables to its device: sets every destination, or none of them when a step fails.  A design-only
+// plan has no device and keeps them null.
+static int upload_tables(const alz_plan* p, std::initializer_list<Upload> tables) {
+  if (p->device < 0) return ALZ_OK;
+  std::vector<void*> got;
+  cudaError_t e = cudaSuccess;
+  for (const Upload& t : tables) {
+    void* d = nullptr;
+    e = cudaMalloc(&d, std::max<size_t>(1, t.bytes));
+    if (e != cudaSuccess) break;
+    got.push_back(d);
+    e = cudaMemcpy(d, t.src, t.bytes, cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) break;
+  }
+  if (e != cudaSuccess) {
+    for (void* d : got) cudaFree(d);
+    return fail(ALZ_ERR_CUDA, "plan upload failed: %s", cudaGetErrorString(e));
+  }
+  size_t i = 0;
+  for (const Upload& t : tables) *t.dst = got[i++];
+  return ALZ_OK;
+}
+
+// ---- the plan's host staging pipeline (alz_apply_f32_host, envelope_host) ---------------------------------------------
+// Creates the pipeline's streams and events on first use.  after_legacy: the ordering contract of include/alz_b200.h for
+// a caller-supplied state, which must be complete or produced by work on the legacy default stream (where torch launches
+// by default): the private pipeline streams are ordered after it.
+static int pipe_open(AlzHostPipe& hp, bool after_legacy) {
+  if (!hp.ready) {
+    for (int i = 0; i < AlzHostPipe::NBUF; ++i) {
+      ALZ_CUDA(cudaStreamCreateWithFlags(&hp.stream[i], cudaStreamNonBlocking));
+      ALZ_CUDA(cudaEventCreateWithFlags(&hp.done[i], cudaEventDisableTiming));
+    }
+    hp.ready = true;
+  }
+  if (after_legacy) {
+    ALZ_CUDA(cudaEventRecord(hp.done[0], cudaStreamLegacy));
+    for (int i = 0; i < AlzHostPipe::NBUF; ++i) ALZ_CUDA(cudaStreamWaitEvent(hp.stream[i], hp.done[0], 0));
+  }
+  return ALZ_OK;
+}
+
+// Grows one staging buffer per pipeline stream to `need` bytes; they are kept in the plan between calls.
+template <class T>
+static int pipe_grow(AlzHostPipe& hp, T** bufs, size_t& have, size_t need) {
+  if (have >= need) return ALZ_OK;
+  for (int i = 0; i < AlzHostPipe::NBUF; ++i) {
+    ALZ_CUDA(cudaStreamSynchronize(hp.stream[i]));
+    cudaFree(bufs[i]);
+    bufs[i] = nullptr;
+  }
+  have = 0;
+  for (int i = 0; i < AlzHostPipe::NBUF; ++i) ALZ_CUDA(cudaMalloc((void**)&bufs[i], need));
+  have = need;
+  return ALZ_OK;
+}
+
+// Waits for every pipeline stream: returns rc, or the first error they report if rc is ALZ_OK.
+static int pipe_finish(AlzHostPipe& hp, int rc) {
+  for (int i = 0; i < AlzHostPipe::NBUF; ++i) {
+    const cudaError_t e = cudaStreamSynchronize(hp.stream[i]);
+    if (e != cudaSuccess && rc == ALZ_OK) rc = fail(ALZ_ERR_CUDA, "pipeline failed: %s", cudaGetErrorString(e));
+  }
+  return rc;
+}
+
+// ---- plan builders, one per kind: the tables of the normalised sections `secs` ([channel][section]) ----
+static int build_biquad(alz_plan* p, const std::vector<std::vector<Sec>>& secs, int Kmax, int nbmax, int nb_rest,
+                        bool headfir, int flags) {
+  const int C = p->C;
+  int K = 8;
+  for (int kk : kBiquadKs) if (kk >= Kmax) { K = kk; break; }
+  if (headfir) K = Kmax == 1 ? 1 : 4;
+  p->kind = ALZ_KIND_BIQUAD;
+  p->K = K;
+  p->NB = headfir ? (nb_rest <= 1 ? 1 : 3) : nbmax;
+  p->NB0 = headfir ? 8 : 0;
+  p->xd = ALZ_H0(p->NB0); p->yd = 2;
+  p->state_doubles = ALZ_STATE_SLOTS(K, p->NB0);
+  // monic only if every b0 is a normal number and the running products stay normal
+  bool monic = !p->parallel_sum;          // ParallelFilter plans keep plain sections: the channel outputs are summed in true units
+  for (int c = 0; c < C && monic; ++c) {
+    double g = 1.0;
+    for (auto& s : secs[c]) {
+      const double b0 = s.b[0];
+      if (!(std::fabs(b0) > 1e-150 && std::fabs(b0) < 1e150)) { monic = false; break; }
+      g *= b0;
+      if (!(std::fabs(g) > 1e-250 && std::fabs(g) < 1e250)) { monic = false; break; }
+    }
+  }
+  // input-side float32 gain (mode 2) when every channel's G is a normal float32 number
+  bool gain_in = monic && !env_int("ALZ_EXACT_GAIN", 0);
+  for (int c = 0; c < C && gain_in; ++c) {
+    double g = 1.0;
+    for (auto& s : secs[c]) g *= s.b[0];
+    if (!(std::fabs(g) > 1e-30 && std::fabs(g) < 1e30)) gain_in = false;
+  }
+  p->monic = monic ? (gain_in ? 2 : 1) : 0;
+  p->fp64_ops = (monic ? K * (p->NB - 1 + 2) + (gain_in ? 0 : 1) : K * (p->NB + 2)) + (headfir ? 8 - p->NB : 0);
+  if (!headfir && !env_int("ALZ_NO_ZMASK", 0)) {   // taps 1 and 2 that no channel has (absent sections count as zero)
+    int zm = (1 << (2 * K)) - 1;
+    for (int c = 0; c < C; ++c)
+      for (size_t k = 0; k < secs[c].size(); ++k)
+        for (int j = 1; j <= 2; ++j)
+          if ((int)secs[c][k].b.size() > j && secs[c][k].b[j] != 0.0) zm &= ~(1 << (2 * (int)k + j - 1));
+    p->zmask = zm;
+    if (K == 4 && p->NB == 3 && (zm & ALZ_ZMASK_KLAPURI) == ALZ_ZMASK_KLAPURI) p->fp64_ops -= 6;   // the kernel that skips them
+  }
+  const int stride = ALZ_COEF_STRIDE(K, p->NB0), nval = ALZ_COEF_NVAL(K, p->NB0);
+  std::vector<double> tab((size_t)C * stride, 0.0);     // channel order, float64 records
+  p->sc.assign((size_t)C * (K + 1), 1.0);
+  for (int c = 0; c < C; ++c) {
+    double* rec = tab.data() + (size_t)c * stride;
+    double g = 1.0, sc = 1.0;
+    if (p->monic == 2) {   // working units start at the (float32-rounded) gain applied to the input
+      double gg = 1.0;
+      for (auto& s : secs[c]) gg *= s.b[0];
+      sc = (double)(float)gg;
+      p->sc[(size_t)c * (K + 1)] = sc;
+    }
+    for (int k = 0; k < K; ++k) {
+      double b[8] = {1.0, 0, 0, 0, 0, 0, 0, 0}, a[3] = {1.0, 0.0, 0.0};   // identity padding
+      if (k < (int)secs[c].size()) {
+        const Sec& s = secs[c][k];
+        b[0] = 0.0;
+        for (size_t i = 0; i < s.b.size(); ++i) b[i] = s.b[i];
+        for (size_t i = 0; i < s.a.size(); ++i) a[i] = s.a[i];
+      }
+      if (k == 0 && p->NB0 == 8)
+        for (int j = 3; j < 8; ++j) rec[5 * K + 1 + (j - 3)] = monic ? b[j] / b[0] : b[j];
+      if (monic) {
+        rec[5 * k + 0] = 1.0;
+        rec[5 * k + 1] = b[1] / b[0];
+        rec[5 * k + 2] = b[2] / b[0];
+        g *= b[0];
+        sc /= b[0];
+      } else {
+        rec[5 * k + 0] = b[0];
+        rec[5 * k + 1] = b[1];
+        rec[5 * k + 2] = b[2];
+      }
+      rec[5 * k + 3] = -a[1];
+      rec[5 * k + 4] = -a[2];
+      p->sc[(size_t)c * (K + 1) + k + 1] = sc;
+    }
+    rec[5 * K] = monic ? g : 1.0;
+  }
+  // ---- precision tier per channel: MEASURED, not guessed -----------------------------------
+  // A channel runs its recurrence in float32 (FP32 pipe, no conversions) only if the float32 core,
+  // executed here on the host with the kernel's own arithmetic, stays within tier_tol of the float64
+  // core on the probe signals; tier_tol defaults to a quarter of the 1e-5 parity bar.  Poles close
+  // to z = 1 (low ERB channels) fail by orders of magnitude and stay in float64.
+  p->tier.assign(C, 0);
+  p->tier_err.assign(C, -1.0);
+  p->tier_tol = env_double("ALZ_TIER_TOL", 2.5e-6);
+  p->probe_len = std::max(64, env_int("ALZ_TIER_PROBE", 8192));
+  const bool tiering = !(flags & ALZ_PLAN_EXACT) && !p->parallel_sum && !env_int("ALZ_NO_FP32_TIER", 0) && p->tier_tol > 0.0;
+  std::vector<double> tab32((size_t)C * stride, 0.0);   // the same records as packed floats
+  for (int c = 0; c < C; ++c) {
+    const double* rec = tab.data() + (size_t)c * stride;
+    float* r32 = reinterpret_cast<float*>(tab32.data() + (size_t)c * stride);
+    bool representable = true;
+    for (int i = 0; i < nval; ++i) {
+      r32[i] = (float)rec[i];
+      if (rec[i] != 0.0 && !(std::fabs(rec[i]) > 1e-30 && std::fabs(rec[i]) < 1e30)) representable = false;
+    }
+    // Near the unit circle float32 state rounding is amplified by ~1 / (1 - r), and on it (a pole cancelled by a zero,
+    // maverage.recursive(1)) the error random-walks with the length of the input, past any probe.
+    double radius = 0.0;
+    for (auto& s : secs[c]) {
+      const double a1 = s.a.size() > 1 ? s.a[1] : 0.0, a2 = s.a.size() > 2 ? s.a[2] : 0.0, disc = a1 * a1 - 4.0 * a2;
+      radius = std::max(radius, disc < 0.0 ? std::sqrt(a2) : 0.5 * (std::fabs(a1) + std::sqrt(disc)));
+    }
+    if (tiering && representable) {
+      p->tier_err[c] = probe_biquad(p, rec, tab32.data() + (size_t)c * stride);
+      if (p->tier_err[c] <= p->tier_tol && radius <= kTierMaxRadius) { p->tier[c] = 1; ++p->n_fp32; }
+    }
+  }
+  if (!p->sequential)
+    for (int c = 0; c < C; ++c) p->chunk_err = std::max(p->chunk_err, chunk_error(secs[c], kChunkProbeLen));
+  // ---- positions: interleave the tiers along blockIdx.x so both kinds of warp share every SM ----
+  {
+    std::vector<int> lst[2];
+    const int order = env_int("ALZ_TIER_ORDER", 1);   // 1: interleave the tiers; 0: channel order; 2: float32 channels first
+    for (int c = 0; c < C; ++c) lst[order == 1 ? p->tier[c] : (order == 2 ? 1 - p->tier[c] : 0)].push_back(c);
+    size_t i0 = 0, i1 = 0;
+    p->pos_channel.clear();
+    while (i0 < lst[0].size() || i1 < lst[1].size()) {   // Bresenham merge: the list that is less consumed goes next
+      const bool take0 = i1 >= lst[1].size() || (i0 < lst[0].size() && i0 * lst[1].size() <= i1 * lst[0].size());
+      p->pos_channel.push_back(take0 ? lst[0][i0++] : lst[1][i1++]);
+    }
+  }
+  p->h_tab.assign((size_t)C * stride, 0.0);
+  for (int pos = 0; pos < C; ++pos) {
+    const int c = p->pos_channel[pos];
+    const std::vector<double>& src = p->tier[c] ? tab32 : tab;
+    double* rec = p->h_tab.data() + (size_t)pos * stride;
+    memcpy(rec, src.data() + (size_t)c * stride, (size_t)nval * sizeof(double));
+    rec[ALZ_COEF_META(K, p->NB0)] = (double)(c + 65536 * p->tier[c]);
+  }
+  p->fp64_ops_exact = p->fp64_ops;
+  // ---- kernel-parameter blocks, built once (launches pass them by address) ---------------------
+  p->coef_small = C * stride <= kCoefSmall;
+  const int ncoef = p->coef_small ? kCoefSmall : kCoefLarge;
+  const int per_launch = ncoef / stride;
+  if (per_launch < 1) return fail(ALZ_ERR_UNSUPPORTED, "coefficient record too large");
+  for (int p0 = 0; p0 < C; p0 += per_launch) {
+    const int npos = std::min(per_launch, C - p0);
+    char* blk = (char*)calloc(1, 2 * sizeof(int) + (size_t)ncoef * sizeof(double));
+    if (!blk) return fail(ALZ_ERR_NOMEM, "out of host memory");
+    reinterpret_cast<int*>(blk)[0] = stride;
+    reinterpret_cast<int*>(blk)[1] = npos;
+    memcpy(blk + 2 * sizeof(int), p->h_tab.data() + (size_t)p0 * stride, (size_t)npos * stride * sizeof(double));
+    p->chunks.push_back({blk, npos});
+  }
+  // Tile group of the launches that fill the machine: 4 (512 B pieces of every output row, 13 CTAs per SM on an H100)
+  // when the arithmetic hides under the output stores; a plan with more FP64 work per channel-sample is bound by
+  // issue and keeps 2, whose 24 CTAs per SM hide more of it.  Measured at the same shape (4096 x 16384,
+  // profiles/h100_tile_group4_ab.txt): klapuri (fp64_ops 10) and slaney (12) gain 3 % with 4, the head-FIR sampled
+  // bank (19) loses 5 %; the bound lies between them.
+  const int group = env_int("ALZ_TILE_GROUP", 0);
+  p->tile_group_forced = group == 1 || group == 2 || group == 4;
+  p->tile_group = p->tile_group_forced ? group : (p->fp64_ops <= kTileGroup4MaxFp64 ? 4 : 2);
+  return ALZ_OK;
+}
+
+// window: one section per channel, dense near taps in registers + prefetched far taps (alz_window.cuh)
+static int build_window(alz_plan* p, const std::vector<std::vector<Sec>>& secs, int nbmax) {
+  const int C = p->C;
+  p->kind = ALZ_KIND_GENERIC;
+  p->window = true;
+  p->K = 1;
+  p->NB = nbmax;
+  p->monic = 0;
+  int near_x = 0, near_y = 0, maxd_x = 0, maxd_y = 0;
+  std::vector<int> far_x, far_y;                    // union over the channels of the taps with delay >= 16
+  for (int c = 0; c < C; ++c) {
+    if (secs[c].empty()) continue;
+    const Sec& s = secs[c][0];
+    for (size_t d = 1; d < s.b.size(); ++d)
+      if (s.b[d] != 0.0) {
+        maxd_x = std::max(maxd_x, (int)d);
+        if (d < 16) near_x = std::max(near_x, (int)d);
+        else if (std::find(far_x.begin(), far_x.end(), (int)d) == far_x.end()) far_x.push_back((int)d);
+      }
+    for (size_t d = 1; d < s.a.size(); ++d)
+      if (s.a[d] != 0.0) {
+        maxd_y = std::max(maxd_y, (int)d);
+        if (d < 16) near_y = std::max(near_y, (int)d);
+        else if (std::find(far_y.begin(), far_y.end(), (int)d) == far_y.end()) far_y.push_back((int)d);
+      }
+  }
+  std::sort(far_x.begin(), far_x.end());
+  std::sort(far_y.begin(), far_y.end());
+  auto slots_of = [](int nearest) { return nearest == 0 ? 0 : (nearest <= 3 ? 4 : 16); };
+  auto pow2 = [](int n) { int q = 1; while (q < n) q <<= 1; return q; };
+  p->win_mx = slots_of(near_x);
+  p->win_my = slots_of(near_y);
+  p->win_nfx = (int)far_x.size();
+  p->win_nfy = (int)far_y.size();
+  int slot = 1;                                     // slot 0: absolute sample count
+  p->win_xwin = slot; slot += p->win_mx ? p->win_mx - 1 : 0;
+  p->win_ywin = slot; slot += p->win_my ? p->win_my - 1 : 0;
+  if (!far_x.empty()) { p->win_xbase = slot; p->win_xmask = pow2(far_x.back() + 16) - 1; slot += p->win_xmask + 1; }
+  if (!far_y.empty()) { p->win_ybase = slot; p->win_ymask = pow2(far_y.back() + 16) - 1; slot += p->win_ymask + 1; }
+  p->xd = maxd_x; p->yd = maxd_y;
+  p->state_doubles = slot;
+  p->fp64_ops = 1 + (p->win_mx ? p->win_mx - 1 : 0) + (p->win_my ? p->win_my - 1 : 0) + p->win_nfx + p->win_nfy;
+  p->win_far_delay = far_x;
+  p->win_far_delay.insert(p->win_far_delay.end(), far_y.begin(), far_y.end());
+  p->h_tab.assign((size_t)C * 32, 0.0);             // [C][b0..b15, -a1..-a15, pad]
+  std::vector<double> fcoef(std::max<size_t>(1, p->win_far_delay.size()) * C, 0.0);
+  for (int c = 0; c < C; ++c) {
+    double* rec = p->h_tab.data() + (size_t)c * 32;
+    if (secs[c].empty()) { rec[0] = 1.0; continue; }   // empty cascade: identity
+    const Sec& s = secs[c][0];
+    for (size_t d = 0; d < s.b.size() && d < 16; ++d) rec[d] = s.b[d];
+    for (size_t d = 1; d < s.a.size() && d < 16; ++d) rec[16 + d - 1] = -s.a[d];
+    for (size_t f = 0; f < far_x.size(); ++f) fcoef[f * C + c] = (size_t)far_x[f] < s.b.size() ? s.b[far_x[f]] : 0.0;
+    for (size_t f = 0; f < far_y.size(); ++f) fcoef[(far_x.size() + f) * C + c] = (size_t)far_y[f] < s.a.size() ? -s.a[far_y[f]] : 0.0;
+  }
+  p->coef_small = C * 32 <= 64;
+  p->win_block = calloc(1, alzi_window_block_bytes(p->coef_small));
+  if (!p->win_block) return fail(ALZ_ERR_NOMEM, "out of host memory");
+  std::vector<int> fd(std::max<size_t>(1, p->win_far_delay.size()), 16);
+  std::copy(p->win_far_delay.begin(), p->win_far_delay.end(), fd.begin());
+  const int rc = upload_tables(p, {table(&p->d_far_delay, fd), table(&p->d_far_coef, fcoef)});
+  if (rc != ALZ_OK) return rc;
+  alzi_window_block_fill(p->win_block, p->coef_small, p->win_nfx, p->win_nfy, p->win_xbase, p->win_xmask, p->win_ybase,
+                         p->win_ymask, p->win_xwin, p->win_ywin, C, p->d_far_delay, p->d_far_coef, p->h_tab.data());
+  return ALZ_OK;
+}
+
+// generic: union tap structure per section
+static int build_generic(alz_plan* p, const std::vector<std::vector<Sec>>& secs, int Kmax, int nbmax) {
+  const int C = p->C;
+  const int K = Kmax;
+  p->kind = ALZ_KIND_GENERIC;
+  p->K = K;
+  p->NB = nbmax;
+  p->monic = 0;
+  std::vector<int> tap_delay;
+  std::vector<std::vector<double>> tap_coef;   // [tap][C]
+  p->h_sec.resize(K);
+  p->h_xlen.assign(K, 0);
+  p->h_ylen.assign(K, 0);
+  int slot = 1;   // slot 0: absolute sample count
+  int ops = 0, xdmax = 0, ydmax = 0;
+  for (int k = 0; k < K; ++k) {
+    size_t nb = 1, na = 1;
+    for (int c = 0; c < C; ++c)
+      if (k < (int)secs[c].size()) { nb = std::max(nb, secs[c][k].b.size()); na = std::max(na, secs[c][k].a.size()); }
+    AlzGenSection gs{};
+    gs.num_begin = (int)tap_delay.size();
+    for (size_t d = 0; d < nb; ++d) {
+      std::vector<double> col(C, 0.0);
+      bool any = false;
+      for (int c = 0; c < C; ++c) {
+        double v;
+        if (k < (int)secs[c].size()) v = d < secs[c][k].b.size() ? secs[c][k].b[d] : 0.0;
+        else v = d == 0 ? 1.0 : 0.0;   // identity padding
+        col[c] = v;
+        any = any || v != 0.0;
+      }
+      if (any || d == 0) { tap_delay.push_back((int)d); tap_coef.push_back(std::move(col)); p->h_tap_is_den.push_back(0); }
+    }
+    gs.nnum = (int)tap_delay.size() - gs.num_begin;
+    gs.den_begin = (int)tap_delay.size();
+    for (size_t d = 1; d < na; ++d) {
+      std::vector<double> col(C, 0.0);
+      bool any = false;
+      for (int c = 0; c < C; ++c) {
+        double v = (k < (int)secs[c].size() && d < secs[c][k].a.size()) ? -secs[c][k].a[d] : 0.0;
+        col[c] = v;
+        any = any || v != 0.0;
+      }
+      if (any) { tap_delay.push_back((int)d); tap_coef.push_back(std::move(col)); p->h_tap_is_den.push_back(1); }
+    }
+    gs.nden = (int)tap_delay.size() - gs.den_begin;
+    const int xlen = (int)nb - 1, ylen = (int)na - 1;
+    auto pow2 = [](int n) { int q = 1; while (q < n) q <<= 1; return q; };
+    if (xlen > 0) { gs.xbase = slot; gs.xmask = pow2(xlen) - 1; slot += gs.xmask + 1; } else { gs.xbase = 0; gs.xmask = -1; }
+    if (ylen > 0) { gs.ybase = slot; gs.ymask = pow2(ylen) - 1; slot += gs.ymask + 1; } else { gs.ybase = 0; gs.ymask = -1; }
+    p->h_sec[k] = gs;
+    p->h_xlen[k] = xlen;
+    p->h_ylen[k] = ylen;
+    xdmax = std::max(xdmax, xlen);
+    ydmax = std::max(ydmax, ylen);
+    ops += gs.nnum + gs.nden;
+  }
+  p->xd = xdmax; p->yd = ydmax;
+  p->state_doubles = slot;
+  p->fp64_ops = ops;
+  const size_t ntaps = tap_delay.size();
+  p->h_tap_delay = tap_delay;
+  std::vector<double> tab(ntaps * C);
+  for (size_t t = 0; t < ntaps; ++t) memcpy(&tab[t * C], tap_coef[t].data(), C * sizeof(double));
+  return upload_tables(p, {table(&p->d_coef, tab), table(&p->d_sec, p->h_sec), table(&p->d_tap_delay, tap_delay)});
+}
+
 // ----------------------------------------------------------------------------------
 extern "C" {
 
@@ -307,9 +706,9 @@ int32_t alz_plan_create_ex(const double* coef, const int32_t* desc, int32_t C, i
   if (!design_only) ALZ_CUDA(cudaGetDevice(&dev));
 
   // ---- normalise every section: divide by a0, trim trailing zeros ------------------
-  struct Sec { std::vector<double> b, a; };   // a[0] == 1 after normalisation (kept for indexing)
   std::vector<std::vector<Sec>> secs(C);
   int Kmax = 0, nbmax = 1, namax = 1;
+  int nb_first = 1, nb_rest = 1;   // numerator taps of the first section vs. of the later ones
   for (int c = 0; c < C; ++c) {
     bool ended = false;
     for (int k = 0; k < KM; ++k) {
@@ -336,13 +735,15 @@ int32_t alz_plan_create_ex(const double* coef, const int32_t* desc, int32_t C, i
       for (double v : s.a) if (!std::isfinite(v)) return fail(ALZ_ERR_INVALID, "non-finite coefficient");
       nbmax = std::max(nbmax, (int)s.b.size());
       namax = std::max(namax, (int)s.a.size());
+      int& nb_max = secs[c].empty() ? nb_first : nb_rest;
+      nb_max = std::max(nb_max, (int)s.b.size());
       secs[c].push_back(std::move(s));
     }
     Kmax = std::max(Kmax, (int)secs[c].size());
   }
   if (Kmax == 0) Kmax = 1;   // bank of empty cascades: identity
 
-  alz_plan* p = new (std::nothrow) alz_plan();
+  std::unique_ptr<alz_plan, void (*)(alz_plan*)> p(new (std::nothrow) alz_plan(), alz_plan_destroy);   // until handed out
   if (!p) return fail(ALZ_ERR_NOMEM, "out of host memory");
   p->C = C;
   p->device = dev;
@@ -363,352 +764,51 @@ int32_t alz_plan_create_ex(const double* coef, const int32_t* desc, int32_t C, i
     }
   p->fr_K = Kmax;
 
-  // numerator taps of the first section vs. of the later ones
-  int nb_first = 1, nb_rest = 1;
-  for (int c = 0; c < C; ++c)
-    for (size_t k = 0; k < secs[c].size(); ++k) {
-      if (k == 0) nb_first = std::max(nb_first, (int)secs[c][k].b.size());
-      else nb_rest = std::max(nb_rest, (int)secs[c][k].b.size());
-    }
   const bool plain = nbmax <= 3 && namax <= 3 && Kmax <= 8;
   const bool headfir = !plain && namax <= 3 && nb_first <= 8 && nb_rest <= 3 && Kmax <= 4;
-  const bool biquad = (plain || headfir) && !(flags & ALZ_PLAN_FORCE_GENERIC);
-  if (biquad) {
-    int K = 8;
-    for (int kk : kBiquadKs) if (kk >= Kmax) { K = kk; break; }
-    if (headfir) K = Kmax == 1 ? 1 : 4;
-    p->kind = ALZ_KIND_BIQUAD;
-    p->K = K;
-    p->NB = headfir ? (nb_rest <= 1 ? 1 : 3) : nbmax;
-    p->NB0 = headfir ? 8 : 0;
-    p->xd = ALZ_H0(p->NB0); p->yd = 2;
-    p->state_doubles = ALZ_STATE_SLOTS(K, p->NB0);
-    // monic only if every b0 is a normal number and the running products stay normal
-    bool monic = !p->parallel_sum;          // ParallelFilter plans keep plain sections: the channel outputs are summed in true units
-    for (int c = 0; c < C && monic; ++c) {
-      double g = 1.0;
-      for (auto& s : secs[c]) {
-        const double b0 = s.b[0];
-        if (!(std::fabs(b0) > 1e-150 && std::fabs(b0) < 1e150)) { monic = false; break; }
-        g *= b0;
-        if (!(std::fabs(g) > 1e-250 && std::fabs(g) < 1e250)) { monic = false; break; }
-      }
-    }
-    // input-side float32 gain (mode 2) when every channel's G is a normal float32 number
-    bool gain_in = monic && !env_int("ALZ_EXACT_GAIN", 0);
-    for (int c = 0; c < C && gain_in; ++c) {
-      double g = 1.0;
-      for (auto& s : secs[c]) g *= s.b[0];
-      if (!(std::fabs(g) > 1e-30 && std::fabs(g) < 1e30)) gain_in = false;
-    }
-    p->monic = monic ? (gain_in ? 2 : 1) : 0;
-    p->fp64_ops = (monic ? K * (p->NB - 1 + 2) + (gain_in ? 0 : 1) : K * (p->NB + 2)) + (headfir ? 8 - p->NB : 0);
-    if (!headfir && !env_int("ALZ_NO_ZMASK", 0)) {   // taps 1 and 2 that no channel has (absent sections count as zero)
-      int zm = (1 << (2 * K)) - 1;
-      for (int c = 0; c < C; ++c)
-        for (size_t k = 0; k < secs[c].size(); ++k)
-          for (int j = 1; j <= 2; ++j)
-            if ((int)secs[c][k].b.size() > j && secs[c][k].b[j] != 0.0) zm &= ~(1 << (2 * (int)k + j - 1));
-      p->zmask = zm;
-      if (K == 4 && p->NB == 3 && (zm & ALZ_ZMASK_KLAPURI) == ALZ_ZMASK_KLAPURI) p->fp64_ops -= 6;   // the kernel that skips them
-    }
-    const int stride = ALZ_COEF_STRIDE(K, p->NB0), nval = ALZ_COEF_NVAL(K, p->NB0);
-    std::vector<double> tab((size_t)C * stride, 0.0);     // channel order, float64 records
-    p->sc.assign((size_t)C * (K + 1), 1.0);
-    for (int c = 0; c < C; ++c) {
-      double* rec = tab.data() + (size_t)c * stride;
-      double g = 1.0, sc = 1.0;
-      if (p->monic == 2) {   // working units start at the (float32-rounded) gain applied to the input
-        double gg = 1.0;
-        for (auto& s : secs[c]) gg *= s.b[0];
-        sc = (double)(float)gg;
-        p->sc[(size_t)c * (K + 1)] = sc;
-      }
-      for (int k = 0; k < K; ++k) {
-        double b[8] = {1.0, 0, 0, 0, 0, 0, 0, 0}, a[3] = {1.0, 0.0, 0.0};   // identity padding
-        if (k < (int)secs[c].size()) {
-          const Sec& s = secs[c][k];
-          b[0] = 0.0;
-          for (size_t i = 0; i < s.b.size(); ++i) b[i] = s.b[i];
-          for (size_t i = 0; i < s.a.size(); ++i) a[i] = s.a[i];
-        }
-        if (k == 0 && p->NB0 == 8)
-          for (int j = 3; j < 8; ++j) rec[5 * K + 1 + (j - 3)] = monic ? b[j] / b[0] : b[j];
-        if (monic) {
-          rec[5 * k + 0] = 1.0;
-          rec[5 * k + 1] = b[1] / b[0];
-          rec[5 * k + 2] = b[2] / b[0];
-          g *= b[0];
-          sc /= b[0];
-        } else {
-          rec[5 * k + 0] = b[0];
-          rec[5 * k + 1] = b[1];
-          rec[5 * k + 2] = b[2];
-        }
-        rec[5 * k + 3] = -a[1];
-        rec[5 * k + 4] = -a[2];
-        p->sc[(size_t)c * (K + 1) + k + 1] = sc;
-      }
-      rec[5 * K] = monic ? g : 1.0;
-    }
-    // ---- precision tier per channel: MEASURED, not guessed -----------------------------------
-    // A channel runs its recurrence in float32 (FP32 pipe, no conversions) only if the float32 core,
-    // executed here on the host with the kernel's own arithmetic, stays within tier_tol of the float64
-    // core on the probe signals; tier_tol defaults to a quarter of the 1e-5 parity bar.  Poles close
-    // to z = 1 (low ERB channels) fail by orders of magnitude and stay in float64.
-    p->tier.assign(C, 0);
-    p->tier_err.assign(C, -1.0);
-    p->tier_tol = env_double("ALZ_TIER_TOL", 2.5e-6);
-    p->probe_len = std::max(64, env_int("ALZ_TIER_PROBE", 8192));
-    const bool tiering = !(flags & ALZ_PLAN_EXACT) && !p->parallel_sum && !env_int("ALZ_NO_FP32_TIER", 0) && p->tier_tol > 0.0;
-    std::vector<double> tab32((size_t)C * stride, 0.0);   // the same records as packed floats
-    for (int c = 0; c < C; ++c) {
-      const double* rec = tab.data() + (size_t)c * stride;
-      float* r32 = reinterpret_cast<float*>(tab32.data() + (size_t)c * stride);
-      bool representable = true;
-      for (int i = 0; i < nval; ++i) {
-        r32[i] = (float)rec[i];
-        if (rec[i] != 0.0 && !(std::fabs(rec[i]) > 1e-30 && std::fabs(rec[i]) < 1e30)) representable = false;
-      }
-      // Near the unit circle float32 state rounding is amplified by ~1 / (1 - r), and on it (a pole cancelled by a zero,
-      // maverage.recursive(1)) the error random-walks with the length of the input, past any probe.
-      double radius = 0.0;
-      for (auto& s : secs[c]) {
-        const double a1 = s.a.size() > 1 ? s.a[1] : 0.0, a2 = s.a.size() > 2 ? s.a[2] : 0.0, disc = a1 * a1 - 4.0 * a2;
-        radius = std::max(radius, disc < 0.0 ? std::sqrt(a2) : 0.5 * (std::fabs(a1) + std::sqrt(disc)));
-      }
-      if (tiering && representable) {
-        p->tier_err[c] = probe_biquad(p, rec, tab32.data() + (size_t)c * stride);
-        if (p->tier_err[c] <= p->tier_tol && radius <= kTierMaxRadius) { p->tier[c] = 1; ++p->n_fp32; }
-      }
-    }
-    if (!p->sequential)
-      for (int c = 0; c < C; ++c) p->chunk_err = std::max(p->chunk_err, chunk_error(secs[c], kChunkProbeLen));
-    // ---- positions: interleave the tiers along blockIdx.x so both kinds of warp share every SM ----
-    {
-      std::vector<int> lst[2];
-      const int order = env_int("ALZ_TIER_ORDER", 1);   // 1: interleave the tiers; 0: channel order; 2: float32 channels first
-      for (int c = 0; c < C; ++c) lst[order == 1 ? p->tier[c] : (order == 2 ? 1 - p->tier[c] : 0)].push_back(c);
-      size_t i0 = 0, i1 = 0;
-      p->pos_channel.clear();
-      while (i0 < lst[0].size() || i1 < lst[1].size()) {   // Bresenham merge: the list that is less consumed goes next
-        const bool take0 = i1 >= lst[1].size() || (i0 < lst[0].size() && i0 * lst[1].size() <= i1 * lst[0].size());
-        p->pos_channel.push_back(take0 ? lst[0][i0++] : lst[1][i1++]);
-      }
-    }
-    p->h_tab.assign((size_t)C * stride, 0.0);
-    for (int pos = 0; pos < C; ++pos) {
-      const int c = p->pos_channel[pos];
-      const std::vector<double>& src = p->tier[c] ? tab32 : tab;
-      double* rec = p->h_tab.data() + (size_t)pos * stride;
-      memcpy(rec, src.data() + (size_t)c * stride, (size_t)nval * sizeof(double));
-      rec[ALZ_COEF_META(K, p->NB0)] = (double)(c + 65536 * p->tier[c]);
-    }
-    p->fp64_ops_exact = p->fp64_ops;
-    // ---- kernel-parameter blocks, built once (launches pass them by address) ---------------------
-    p->coef_small = C * stride <= kCoefSmall;
-    const int ncoef = p->coef_small ? kCoefSmall : kCoefLarge;
-    const int per_launch = ncoef / stride;
-    if (per_launch < 1) { alz_plan_destroy(p); return fail(ALZ_ERR_UNSUPPORTED, "coefficient record too large"); }
-    for (int p0 = 0; p0 < C; p0 += per_launch) {
-      const int npos = std::min(per_launch, C - p0);
-      char* blk = (char*)calloc(1, 2 * sizeof(int) + (size_t)ncoef * sizeof(double));
-      if (!blk) { alz_plan_destroy(p); return fail(ALZ_ERR_NOMEM, "out of host memory"); }
-      reinterpret_cast<int*>(blk)[0] = stride;
-      reinterpret_cast<int*>(blk)[1] = npos;
-      memcpy(blk + 2 * sizeof(int), p->h_tab.data() + (size_t)p0 * stride, (size_t)npos * stride * sizeof(double));
-      p->chunks.push_back({blk, npos});
-    }
-    // Tile group of the launches that fill the machine: 4 (512 B pieces of every output row, 13 CTAs per SM on an H100)
-    // when the arithmetic hides under the output stores; a plan with more FP64 work per channel-sample is bound by
-    // issue and keeps 2, whose 24 CTAs per SM hide more of it.  Measured at the same shape (4096 x 16384,
-    // profiles/h100_tile_group4_ab.txt): klapuri (fp64_ops 10) and slaney (12) gain 3 % with 4, the head-FIR sampled
-    // bank (19) loses 5 %; the bound lies between them.
-    const int group = env_int("ALZ_TILE_GROUP", 0);
-    p->tile_group_forced = group == 1 || group == 2 || group == 4;
-    p->tile_group = p->tile_group_forced ? group : (p->fp64_ops <= kTileGroup4MaxFp64 ? 4 : 2);
-  } else if (Kmax == 1 && !(flags & ALZ_PLAN_FORCE_GENERIC) && C * 32 <= kCoefLarge && !env_int("ALZ_NO_WINDOW", 0)) {
-    // ---- window: one section per channel, dense near taps in registers + prefetched far taps (alz_window.cuh) ----
-    p->kind = ALZ_KIND_GENERIC;
-    p->window = true;
-    p->K = 1;
-    p->NB = nbmax;
-    p->monic = 0;
-    int near_x = 0, near_y = 0, maxd_x = 0, maxd_y = 0;
-    std::vector<int> far_x, far_y;                    // union over the channels of the taps with delay >= 16
-    for (int c = 0; c < C; ++c) {
-      if (secs[c].empty()) continue;
-      const Sec& s = secs[c][0];
-      for (size_t d = 1; d < s.b.size(); ++d)
-        if (s.b[d] != 0.0) {
-          maxd_x = std::max(maxd_x, (int)d);
-          if (d < 16) near_x = std::max(near_x, (int)d);
-          else if (std::find(far_x.begin(), far_x.end(), (int)d) == far_x.end()) far_x.push_back((int)d);
-        }
-      for (size_t d = 1; d < s.a.size(); ++d)
-        if (s.a[d] != 0.0) {
-          maxd_y = std::max(maxd_y, (int)d);
-          if (d < 16) near_y = std::max(near_y, (int)d);
-          else if (std::find(far_y.begin(), far_y.end(), (int)d) == far_y.end()) far_y.push_back((int)d);
-        }
-    }
-    std::sort(far_x.begin(), far_x.end());
-    std::sort(far_y.begin(), far_y.end());
-    auto slots_of = [](int nearest) { return nearest == 0 ? 0 : (nearest <= 3 ? 4 : 16); };
-    auto pow2 = [](int n) { int q = 1; while (q < n) q <<= 1; return q; };
-    p->win_mx = slots_of(near_x);
-    p->win_my = slots_of(near_y);
-    p->win_nfx = (int)far_x.size();
-    p->win_nfy = (int)far_y.size();
-    int slot = 1;                                     // slot 0: absolute sample count
-    p->win_xwin = slot; slot += p->win_mx ? p->win_mx - 1 : 0;
-    p->win_ywin = slot; slot += p->win_my ? p->win_my - 1 : 0;
-    if (!far_x.empty()) { p->win_xbase = slot; p->win_xmask = pow2(far_x.back() + 16) - 1; slot += p->win_xmask + 1; }
-    if (!far_y.empty()) { p->win_ybase = slot; p->win_ymask = pow2(far_y.back() + 16) - 1; slot += p->win_ymask + 1; }
-    p->xd = maxd_x; p->yd = maxd_y;
-    p->state_doubles = slot;
-    p->fp64_ops = 1 + (p->win_mx ? p->win_mx - 1 : 0) + (p->win_my ? p->win_my - 1 : 0) + p->win_nfx + p->win_nfy;
-    p->win_far_delay = far_x;
-    p->win_far_delay.insert(p->win_far_delay.end(), far_y.begin(), far_y.end());
-    p->h_tab.assign((size_t)C * 32, 0.0);             // [C][b0..b15, -a1..-a15, pad]
-    std::vector<double> fcoef(std::max<size_t>(1, p->win_far_delay.size()) * C, 0.0);
-    for (int c = 0; c < C; ++c) {
-      double* rec = p->h_tab.data() + (size_t)c * 32;
-      if (secs[c].empty()) { rec[0] = 1.0; continue; }   // empty cascade: identity
-      const Sec& s = secs[c][0];
-      for (size_t d = 0; d < s.b.size() && d < 16; ++d) rec[d] = s.b[d];
-      for (size_t d = 1; d < s.a.size() && d < 16; ++d) rec[16 + d - 1] = -s.a[d];
-      for (size_t f = 0; f < far_x.size(); ++f) fcoef[f * C + c] = (size_t)far_x[f] < s.b.size() ? s.b[far_x[f]] : 0.0;
-      for (size_t f = 0; f < far_y.size(); ++f) fcoef[(far_x.size() + f) * C + c] = (size_t)far_y[f] < s.a.size() ? -s.a[far_y[f]] : 0.0;
-    }
-    p->coef_small = C * 32 <= 64;
-    p->win_block = calloc(1, alzi_window_block_bytes(p->coef_small));
-    if (!p->win_block) { alz_plan_destroy(p); return fail(ALZ_ERR_NOMEM, "out of host memory"); }
-    if (!design_only) {
-      const size_t nf = std::max<size_t>(1, p->win_far_delay.size());
-      std::vector<int> fd(nf, 16);
-      std::copy(p->win_far_delay.begin(), p->win_far_delay.end(), fd.begin());
-      cudaError_t e = cudaMalloc(&p->d_far_delay, nf * sizeof(int));
-      if (e == cudaSuccess) e = cudaMemcpy(p->d_far_delay, fd.data(), nf * sizeof(int), cudaMemcpyHostToDevice);
-      if (e == cudaSuccess) e = cudaMalloc(&p->d_far_coef, fcoef.size() * sizeof(double));
-      if (e == cudaSuccess) e = cudaMemcpy(p->d_far_coef, fcoef.data(), fcoef.size() * sizeof(double), cudaMemcpyHostToDevice);
-      if (e != cudaSuccess) { alz_plan_destroy(p); return fail(ALZ_ERR_CUDA, "plan upload failed: %s", cudaGetErrorString(e)); }
-    }
-    alzi_window_block_fill(p->win_block, p->coef_small, p->win_nfx, p->win_nfy, p->win_xbase, p->win_xmask, p->win_ybase,
-                           p->win_ymask, p->win_xwin, p->win_ywin, C, p->d_far_delay, p->d_far_coef, p->h_tab.data());
-  } else {
-    // ---- generic: union tap structure per section --------------------------------
-    const int K = Kmax;
-    p->kind = ALZ_KIND_GENERIC;
-    p->K = K;
-    p->NB = nbmax;
-    p->monic = 0;
-    std::vector<int> tap_delay;
-    std::vector<std::vector<double>> tap_coef;   // [tap][C]
-    p->h_sec.resize(K);
-    p->h_xlen.assign(K, 0);
-    p->h_ylen.assign(K, 0);
-    int slot = 1;   // slot 0: absolute sample count
-    int ops = 0, xdmax = 0, ydmax = 0;
-    for (int k = 0; k < K; ++k) {
-      size_t nb = 1, na = 1;
-      for (int c = 0; c < C; ++c)
-        if (k < (int)secs[c].size()) { nb = std::max(nb, secs[c][k].b.size()); na = std::max(na, secs[c][k].a.size()); }
-      AlzGenSection gs{};
-      gs.num_begin = (int)tap_delay.size();
-      for (size_t d = 0; d < nb; ++d) {
-        std::vector<double> col(C, 0.0);
-        bool any = false;
-        for (int c = 0; c < C; ++c) {
-          double v;
-          if (k < (int)secs[c].size()) v = d < secs[c][k].b.size() ? secs[c][k].b[d] : 0.0;
-          else v = d == 0 ? 1.0 : 0.0;   // identity padding
-          col[c] = v;
-          any = any || v != 0.0;
-        }
-        if (any || d == 0) { tap_delay.push_back((int)d); tap_coef.push_back(std::move(col)); p->h_tap_is_den.push_back(0); }
-      }
-      gs.nnum = (int)tap_delay.size() - gs.num_begin;
-      gs.den_begin = (int)tap_delay.size();
-      for (size_t d = 1; d < na; ++d) {
-        std::vector<double> col(C, 0.0);
-        bool any = false;
-        for (int c = 0; c < C; ++c) {
-          double v = (k < (int)secs[c].size() && d < secs[c][k].a.size()) ? -secs[c][k].a[d] : 0.0;
-          col[c] = v;
-          any = any || v != 0.0;
-        }
-        if (any) { tap_delay.push_back((int)d); tap_coef.push_back(std::move(col)); p->h_tap_is_den.push_back(1); }
-      }
-      gs.nden = (int)tap_delay.size() - gs.den_begin;
-      const int xlen = (int)nb - 1, ylen = (int)na - 1;
-      auto pow2 = [](int n) { int q = 1; while (q < n) q <<= 1; return q; };
-      if (xlen > 0) { gs.xbase = slot; gs.xmask = pow2(xlen) - 1; slot += gs.xmask + 1; } else { gs.xbase = 0; gs.xmask = -1; }
-      if (ylen > 0) { gs.ybase = slot; gs.ymask = pow2(ylen) - 1; slot += gs.ymask + 1; } else { gs.ybase = 0; gs.ymask = -1; }
-      p->h_sec[k] = gs;
-      p->h_xlen[k] = xlen;
-      p->h_ylen[k] = ylen;
-      xdmax = std::max(xdmax, xlen);
-      ydmax = std::max(ydmax, ylen);
-      ops += gs.nnum + gs.nden;
-    }
-    p->xd = xdmax; p->yd = ydmax;
-    p->state_doubles = slot;
-    p->fp64_ops = ops;
-    const size_t ntaps = tap_delay.size();
-    p->h_tap_delay = tap_delay;
-    std::vector<double> tab(ntaps * C);
-    for (size_t t = 0; t < ntaps; ++t) memcpy(&tab[t * C], tap_coef[t].data(), C * sizeof(double));
-    cudaError_t e = design_only ? cudaSuccess : cudaMalloc(&p->d_coef, tab.size() * sizeof(double));
-    if (design_only) { *out = p; return ALZ_OK; }
-    if (e == cudaSuccess) e = cudaMemcpy(p->d_coef, tab.data(), tab.size() * sizeof(double), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMalloc(&p->d_sec, K * sizeof(AlzGenSection));
-    if (e == cudaSuccess) e = cudaMemcpy(p->d_sec, p->h_sec.data(), K * sizeof(AlzGenSection), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMalloc(&p->d_tap_delay, ntaps * sizeof(int));
-    if (e == cudaSuccess) e = cudaMemcpy(p->d_tap_delay, tap_delay.data(), ntaps * sizeof(int), cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) { alz_plan_destroy(p); return fail(ALZ_ERR_CUDA, "plan upload failed: %s", cudaGetErrorString(e)); }
-  }
-  *out = p;
+  const bool generic = (flags & ALZ_PLAN_FORCE_GENERIC) != 0;
+  int rc;
+  if ((plain || headfir) && !generic)
+    rc = build_biquad(p.get(), secs, Kmax, nbmax, nb_rest, headfir, flags);
+  else if (Kmax == 1 && !generic && C * 32 <= kCoefLarge && !env_int("ALZ_NO_WINDOW", 0))
+    rc = build_window(p.get(), secs, nbmax);
+  else
+    rc = build_generic(p.get(), secs, Kmax, nbmax);
+  if (rc != ALZ_OK) return rc;
+  *out = p.release();
   return ALZ_OK;
 }
 
 void alz_plan_destroy(alz_plan* p) {
   if (!p) return;
-  if (p->device < 0) {   // design-only: host tables only
-    for (auto& ch : p->chunks) free(ch.block);
-    free(p->win_block);
-    delete p;
-    return;
-  }
-  int cur = 0;
-  cudaGetDevice(&cur);
-  cudaSetDevice(p->device);
-  // Launches on any stream may still read the tables freed below (the window and generic kernels read d_coef, d_sec,
-  // d_tap_delay and d_far_* from global memory, the scans the cached M): cudaFree only "may perform implicit
-  // synchronization", so wait for the device (its green contexts included) first.
-  cudaDeviceSynchronize();
-  if (p->pipe.ready) {
-    for (int i = 0; i < AlzHostPipe::NBUF; ++i) {
-      if (p->pipe.stream[i]) { cudaStreamSynchronize(p->pipe.stream[i]); cudaStreamDestroy(p->pipe.stream[i]); }
-      if (p->pipe.done[i]) cudaEventDestroy(p->pipe.done[i]);
-      cudaFree(p->pipe.dx[i]);
-      cudaFree(p->pipe.dy[i]);
-      cudaFree(p->pipe.dst[i]);
-      cudaFree(p->pipe.des[i]);
+  if (p->device >= 0) {   // a design-only plan holds host tables only
+    DeviceScope dev(p->device);
+    // Launches on any stream may still read the tables freed below (the window and generic kernels read d_coef, d_sec,
+    // d_tap_delay and d_far_* from global memory, the scans the cached M): cudaFree only "may perform implicit
+    // synchronization", so wait for the device (its green contexts included) first.
+    cudaDeviceSynchronize();
+    if (p->pipe.ready) {
+      for (int i = 0; i < AlzHostPipe::NBUF; ++i) {
+        if (p->pipe.stream[i]) { cudaStreamSynchronize(p->pipe.stream[i]); cudaStreamDestroy(p->pipe.stream[i]); }
+        if (p->pipe.done[i]) cudaEventDestroy(p->pipe.done[i]);
+        cudaFree(p->pipe.dx[i]);
+        cudaFree(p->pipe.dy[i]);
+        cudaFree(p->pipe.dst[i]);
+        cudaFree(p->pipe.des[i]);
+      }
     }
+    for (auto* e : p->m_cache) { cudaFree(e->M); cudaEventDestroy(e->ready); delete e; }
+    cudaFree(p->d_far_delay);
+    cudaFree(p->d_far_coef);
+    cudaFree(p->d_coef);
+    cudaFree(p->d_sec);
+    cudaFree(p->d_tap_delay);
+    cudaFree(p->d_fr_coef);
+    cudaFree(p->d_fr_desc);
+    cudaGetLastError();
   }
   for (auto& ch : p->chunks) free(ch.block);
-  for (auto* e : p->m_cache) { cudaFree(e->M); cudaEventDestroy(e->ready); delete e; }
   free(p->win_block);
-  cudaFree(p->d_far_delay);
-  cudaFree(p->d_far_coef);
-  cudaFree(p->d_coef);
-  cudaFree(p->d_sec);
-  cudaFree(p->d_tap_delay);
-  cudaFree(p->d_fr_coef);
-  cudaFree(p->d_fr_desc);
-  cudaSetDevice(cur);
-  cudaGetLastError();
   delete p;
 }
 
@@ -766,6 +866,8 @@ int32_t alz_state_init(const alz_plan* p, double* state, int64_t S, const double
   if (p->device < 0) return fail(ALZ_ERR_CUDA, "design-only plan: no device");
   if (S == 0) return ALZ_OK;
   if (!state) return fail(ALZ_ERR_INVALID, "state is null");
+  DeviceScope dev(p->device);
+  ALZ_CUDA(dev.status);
   cudaStream_t st = (cudaStream_t)cuda_stream;
   const long long R = (long long)S * p->C;
   const size_t bytes = (size_t)p->state_doubles * R * sizeof(double);
@@ -818,14 +920,13 @@ int32_t alz_state_init(const alz_plan* p, double* state, int64_t S, const double
         }
       }
   }
-  double* d_proto = nullptr;
-  ALZ_CUDA(cudaMallocAsync((void**)&d_proto, proto.size() * sizeof(double), st));
-  ALZ_CUDA(cudaMemcpyAsync(d_proto, proto.data(), proto.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+  StreamScratch<double> d_proto(st);
+  ALZ_CUDA(d_proto.alloc(proto.size()));
+  ALZ_CUDA(cudaMemcpyAsync(d_proto.ptr, proto.data(), proto.size() * sizeof(double), cudaMemcpyHostToDevice, st));
   const long long n = R * slots;
-  alz_state_fill_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(state, d_proto, R, C, slots);
+  alz_state_fill_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(state, d_proto.ptr, R, C, slots);
   ALZ_CUDA(cudaGetLastError());
   g_launches.fetch_add(1, std::memory_order_relaxed);
-  ALZ_CUDA(cudaFreeAsync(d_proto, st));
   ALZ_CUDA(cudaStreamSynchronize(st));   // proto (pageable host vector) must be consumed before return
   return ALZ_OK;
 }
@@ -892,13 +993,6 @@ static __global__ void __launch_bounds__(32) alz_chunk_scan_kernel(const double*
     cur = a0 + a1;
   }
   if (on) *us = cur;
-}
-
-static int apply_impl(const alz_plan* p, const float* x, float* y, double* state, long long sstride, long long S,
-                      long long T, long long xs, long long ys, cudaStream_t st, const double* tv, long long tv_stride, long long ysS);
-static int apply_plain(const alz_plan* p, const float* x, float* y, double* state, long long sstride, long long S,
-                       long long T, long long xs, long long ys, cudaStream_t st) {
-  return apply_impl(p, x, y, state, sstride, S, T, xs, ys, st, nullptr, 0, 0);
 }
 
 // Time-parallel evaluation pays when the plain launch (one warp per channel and 32 streams, serial in time)
@@ -983,26 +1077,24 @@ static int chunk_transition(const alz_plan* p, long long L, cudaStream_t st, alz
       ++e->users;
     } else {   // basis run: L zero samples from each unit state -> M = A^L, per channel (it does not depend on the stream)
       double* M = nullptr;
-      float *xz = nullptr, *ydum = nullptr;
+      StreamScratch<float> xz(st), ydum(st);
       cudaEvent_t ready = nullptr;
       ALZ_CUDA(cudaMalloc((void**)&M, (size_t)d * d * C * 8));
       cudaError_t ce = cudaEventCreateWithFlags(&ready, cudaEventDisableTiming);
-      if (ce == cudaSuccess) ce = cudaMallocAsync((void**)&xz, (size_t)d * L * 4, st);
-      if (ce == cudaSuccess) ce = cudaMallocAsync((void**)&ydum, (size_t)d * C * L * 4, st);
-      if (ce == cudaSuccess) ce = cudaMemsetAsync(xz, 0, (size_t)d * L * 4, st);
+      if (ce == cudaSuccess) ce = xz.alloc((size_t)d * L);
+      if (ce == cudaSuccess) ce = ydum.alloc((size_t)d * C * L);
+      if (ce == cudaSuccess) ce = cudaMemsetAsync(xz.ptr, 0, (size_t)d * L * 4, st);
       int rc = ALZ_OK;
       if (ce == cudaSuccess) {
         const long long n = (long long)d * d * C;
         alz_unit_state_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(M, d, C);
         g_launches.fetch_add(1, std::memory_order_relaxed);
         AlzTileArgs tb{};
-        tb.x = xz; tb.y = ydum; tb.S = d; tb.T = L; tb.xs = L; tb.ys = L; tb.ysS = (long long)C * L; tb.C = C; tb.Stot = d;
+        tb.x = xz.ptr; tb.y = ydum.ptr; tb.S = d; tb.T = L; tb.xs = L; tb.ys = L; tb.ysS = (long long)C * L; tb.C = C; tb.Stot = d;
         tb.vec_in = tb.vec_out = 1;
         tb.exp = 2;                                                             // its outputs are not needed: no tile stores
         rc = apply_launch(p, tb, M, (long long)d * C, st, nullptr, 0);
       }
-      if (xz) cudaFreeAsync(xz, st);
-      if (ydum) cudaFreeAsync(ydum, st);
       if (ce == cudaSuccess && rc == ALZ_OK) ce = cudaEventRecord(ready, st);
       if (ce != cudaSuccess || rc != ALZ_OK) {
         cudaStreamSynchronize(st);                 // the basis run may be queued: M stays allocated until it is done
@@ -1038,51 +1130,61 @@ static int vec_out_ok(const float* y, long long ys, long long ysS) {
   return (((uintptr_t)y & 15) == 0 && (ys & 3) == 0 && (ysS & 3) == 0) ? 1 : 0;
 }
 
-static int apply_chunked(const alz_plan* p, const float* x, float* y, double* state, long long sstride, long long S,
-                         long long T, long long xs, long long ys, long long P, long long L, cudaStream_t st) {
+// Pass 1 and the bank-state scan of the time-parallel evaluation, on the caller's virtual streams `ta` (P chunks of L
+// samples per stream): every chunk runs from a zero state into `zero`, and the scan turns those final states into
+// every chunk's true initial state, in `init` ([slot][V * C] each, allocated here), and carries `state` past the last
+// chunk.  `zero` is free for other use afterwards.
+static int chunk_states(const alz_plan* p, AlzTileArgs ta, double* state, long long sstride, long long P, long long L,
+                        cudaStream_t st, StreamScratch<double>& zero, StreamScratch<double>& init) {
   const int C = p->C, d = p->state_doubles;
-  const long long Tmain = P * L, V = S * P;        // V virtual streams
+  const long long V = ta.S, S = V / P;
   const size_t nstate = (size_t)d * V * C;
   keep_async_pool();
-  double *Z1 = nullptr, *Z2 = nullptr;
+  ALZ_CUDA(zero.alloc(nstate));
+  ALZ_CUDA(init.alloc(nstate));
+  ALZ_CUDA(cudaMemsetAsync(zero.ptr, 0, nstate * 8, st));
   alz_plan::MEntry* m = nullptr;
-  ALZ_CUDA(cudaMallocAsync((void**)&Z1, nstate * 8, st));
-  ALZ_CUDA(cudaMallocAsync((void**)&Z2, nstate * 8, st));
-  ALZ_CUDA(cudaMemsetAsync(Z1, 0, nstate * 8, st));
   int rc = chunk_transition(p, L, st, &m);
+  if (rc != ALZ_OK) return rc;
+  ta.exp = 2;                                      // zero-state chunks: only the final states matter, no tile stores
+  rc = apply_launch(p, ta, zero.ptr, V * C, st, nullptr, 0);
+  if (rc == ALZ_OK) {
+    alz_chunk_scan_kernel<<<dim3((unsigned)C, (unsigned)S), 32, 0, st>>>(zero.ptr, init.ptr, m->M, state, sstride, sstride / C,
+                                                                         d, C, S, P);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) rc = fail(ALZ_ERR_CUDA, "chunk scan launch failed: %s", cudaGetErrorString(e));
+    else g_launches.fetch_add(1, std::memory_order_relaxed);
+  }
+  chunk_release(p, m);
+  return rc;
+}
+
+// The first P * L samples of every stream, time-parallel.
+static int apply_chunked(const alz_plan* p, const float* x, float* y, double* state, long long sstride, long long S,
+                         long long xs, long long ys, long long P, long long L, cudaStream_t st) {
+  const int C = p->C;
+  const long long V = S * P;                       // V virtual streams
   AlzTileArgs ta{};
   ta.x = x; ta.y = y; ta.S = V; ta.T = L; ta.xs = xs; ta.ys = ys; ta.ysS = (long long)C * ys; ta.C = C; ta.Stot = V;
   ta.vec_in = (((uintptr_t)x & 15) == 0 && (xs & 3) == 0) ? 1 : 0;          // L is a multiple of 32: chunk starts keep the alignment
   ta.vec_out = vec_out_ok(y, ys, ta.ysS);
   ta.vP = (int)P;
-  if (rc == ALZ_OK) {
-    ta.exp = 2;                                                                 // pass 1: zero-state chunks, only the final states matter
-    rc = apply_launch(p, ta, Z1, V * C, st, nullptr, 0);
-  }
-  if (rc == ALZ_OK) {
-    alz_chunk_scan_kernel<<<dim3((unsigned)C, (unsigned)S), 32, 0, st>>>(Z1, Z2, m->M, state, sstride, sstride / C, d, C, S, P);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) rc = fail(ALZ_ERR_CUDA, "chunk scan launch failed: %s", cudaGetErrorString(e));
-  }
-  if (m) chunk_release(p, m);
-  if (rc == ALZ_OK) {
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    ta.exp = 0;
-    rc = apply_launch(p, ta, Z2, V * C, st, nullptr, 0);                        // pass 2: every chunk from its true initial state
-  }
-  cudaFreeAsync(Z1, st); cudaFreeAsync(Z2, st);
-  if (rc == ALZ_OK && T > Tmain)                                                // left-over samples of all streams: the same decision again
-    rc = apply_plain(p, x + Tmain, y + Tmain, state, sstride, S, T - Tmain, xs, ys, st);
-  return rc;
+  StreamScratch<double> zero(st), init(st);
+  const int rc = chunk_states(p, ta, state, sstride, P, L, st, zero, init);
+  if (rc != ALZ_OK) return rc;
+  return apply_launch(p, ta, init.ptr, V * C, st, nullptr, 0);              // pass 2: every chunk from its true initial state
 }
 
+// ysS: the distance between the output rows of consecutive streams.
 static int apply_impl(const alz_plan* p, const float* x, float* y, double* state, long long sstride, long long S,
-                      long long T, long long xs, long long ys, cudaStream_t st, const double* tv,
-                      long long tv_stride, long long ysS) {
-  if (ysS == 0) ysS = (long long)p->C * ys;
+                      long long T, long long xs, long long ys, long long ysS, cudaStream_t st, const double* tv = nullptr,
+                      long long tv_stride = 0) {
   long long P = 0, L = 0;
-  if (!tv && ysS == (long long)p->C * ys && chunk_geometry(p, S, T, 2, &P, &L))
-    return apply_chunked(p, x, y, state, sstride, S, T, xs, ys, P, L, st);
+  while (!tv && ysS == (long long)p->C * ys && chunk_geometry(p, S, T, 2, &P, &L)) {
+    const int rc = apply_chunked(p, x, y, state, sstride, S, xs, ys, P, L, st);
+    if (rc != ALZ_OK || T == P * L) return rc;
+    x += P * L; y += P * L; T -= P * L;            // left-over samples of all streams: the same decision again
+  }
   AlzTileArgs ta{};
   ta.T = T; ta.xs = xs; ta.ys = ys; ta.ysS = ysS; ta.C = p->C;
   ta.Stot = sstride / p->C;
@@ -1100,39 +1202,37 @@ static int apply_impl(const alz_plan* p, const float* x, float* y, double* state
   return ALZ_OK;
 }
 
+// The argument checks of the apply-style entries, in this order.  False when the entry returns *rc at once: an error, or
+// ALZ_OK for an empty block.  `buffers`: every buffer the entry needs is given.  `need_device`: a design-only plan is
+// refused before the sizes are looked at.
+static bool apply_check(const alz_plan* p, bool need_device, int64_t S, int64_t T, bool buffers, int64_t xs, int64_t ys,
+                        int* rc) {
+  *rc = ALZ_OK;
+  if (!p) *rc = fail(ALZ_ERR_INVALID, "plan is null");
+  else if (need_device && p->device < 0) *rc = fail(ALZ_ERR_CUDA, "design-only plan: no device");
+  else if (S < 0 || T < 0) *rc = fail(ALZ_ERR_INVALID, "negative size");
+  else if (S == 0 || T == 0) return false;
+  else if (!buffers) *rc = fail(ALZ_ERR_INVALID, "null buffer");
+  else if (xs < T || ys < T) *rc = fail(ALZ_ERR_INVALID, "row stride shorter than n_samples");
+  return *rc == ALZ_OK;
+}
+
 int32_t alz_apply_f32(const alz_plan* p, const float* x, float* y, double* state, int64_t S, int64_t T,
                       int64_t xs, int64_t ys, void* cuda_stream) {
   if (!p) return fail(ALZ_ERR_INVALID, "plan is null");
-  if (p->device < 0) return fail(ALZ_ERR_CUDA, "design-only plan: no device");
-  if (S < 0 || T < 0) return fail(ALZ_ERR_INVALID, "negative size");
-  if (S == 0 || T == 0) return ALZ_OK;
-  if (!x || !y || !state) return fail(ALZ_ERR_INVALID, "null buffer");
-  if (xs < T || ys < T) return fail(ALZ_ERR_INVALID, "row stride shorter than n_samples");
-  int cur = -1;
-  ALZ_CUDA(cudaGetDevice(&cur));
-  if (cur != p->device) ALZ_CUDA(cudaSetDevice(p->device));
-  const int rc = apply_plain(p, x, y, state, (long long)S * p->C, S, T, xs, ys, (cudaStream_t)cuda_stream);
-  if (cur != p->device) cudaSetDevice(cur);
-  return rc;
+  return alz_apply_f32_ex(p, x, y, state, S, T, xs, ys, (int64_t)p->C * ys, cuda_stream);
 }
 
 int32_t alz_apply_f32_ex(const alz_plan* p, const float* x, float* y, double* state, int64_t S, int64_t T,
                          int64_t xs, int64_t ys, int64_t y_stream_stride, void* cuda_stream) {
-  if (!p) return fail(ALZ_ERR_INVALID, "plan is null");
-  if (p->device < 0) return fail(ALZ_ERR_CUDA, "design-only plan: no device");
-  if (S < 0 || T < 0) return fail(ALZ_ERR_INVALID, "negative size");
-  if (S == 0 || T == 0) return ALZ_OK;
-  if (!x || !y || !state) return fail(ALZ_ERR_INVALID, "null buffer");
-  if (xs < T || ys < T) return fail(ALZ_ERR_INVALID, "row stride shorter than n_samples");
+  int rc;
+  if (!apply_check(p, true, S, T, x && y && state, xs, ys, &rc)) return rc;
   // rows must not overlap: stream-major (stream stride >= C rows) or channel-major (row stride >= S stream strides)
   if (y_stream_stride < T || !(y_stream_stride >= (int64_t)p->C * ys || ys >= S * y_stream_stride))
     return fail(ALZ_ERR_INVALID, "output rows overlap: need y_stream_stride >= n_channels * y_stride or y_stride >= n_streams * y_stream_stride");
-  int cur = -1;
-  ALZ_CUDA(cudaGetDevice(&cur));
-  if (cur != p->device) ALZ_CUDA(cudaSetDevice(p->device));
-  const int rc = apply_impl(p, x, y, state, (long long)S * p->C, S, T, xs, ys, (cudaStream_t)cuda_stream, nullptr, 0, y_stream_stride);
-  if (cur != p->device) cudaSetDevice(cur);
-  return rc;
+  DeviceScope dev(p->device);
+  ALZ_CUDA(dev.status);
+  return apply_impl(p, x, y, state, (long long)S * p->C, S, T, xs, ys, y_stream_stride, (cudaStream_t)cuda_stream);
 }
 
 // ---- the bank with the fused envelope consumer ----------------------------------------------------------------------
@@ -1143,9 +1243,6 @@ static int envelope_launch(const alz_plan* p, const AlzTileArgs& ta, cudaStream_
   return p->NB0 == 8 ? alzi_launch_envelope_headfir_k4(p, ta, st) : alzi_launch_envelope_k4(p, ta, st);
 }
 
-static int envelope_impl(const alz_plan* p, const float* x, float* env, double* state, double* env_state, long long sstride,
-                         long long S, long long T, long long xs, long long es, const EnvParams& ep, cudaStream_t st);
-
 // Time-parallel evaluation of few long streams (the bank's is apply_chunked): every stream is cut into P chunks of L
 // samples (virtual streams), and
 //   pass 1  the bank runs every chunk from a zero state, no output                     -> F_p
@@ -1155,80 +1252,62 @@ static int envelope_impl(const alz_plan* p, const float* x, float* env, double* 
 //           e_{p+1} = Fe_p + R^L e_p, the same affine scan with a one-value state        -> the chunks' true lowpass states
 //   pass 3  bank and lowpass from their true states, values stored at each chunk's decimation phase and offset
 // and the T - P L samples left over continue sequentially.  Exact in exact arithmetic; in float64 the chunk states
-// differ from the sequential ones by rounding only.
+// differ from the sequential ones by rounding only.  This evaluates the first P L samples of every stream.
 static int envelope_chunked(const alz_plan* p, const float* x, float* env, double* state, double* env_state, long long sstride,
-                            long long S, long long T, long long xs, long long es, const EnvParams& ep, long long P, long long L,
+                            long long S, long long xs, long long es, const EnvParams& ep, long long P, long long L,
                             cudaStream_t st) {
-  const int C = p->C, d = p->state_doubles;
-  const long long Tmain = P * L, V = S * P;        // V virtual streams
-  const size_t nstate = (size_t)d * V * C, nenv = (size_t)V * C;
-  keep_async_pool();
-  double *Z1 = nullptr, *Z2 = nullptr, *E = nullptr, *E2 = nullptr, *RL = nullptr;
-  alz_plan::MEntry* m = nullptr;
-  ALZ_CUDA(cudaMallocAsync((void**)&Z1, nstate * 8, st));
-  ALZ_CUDA(cudaMallocAsync((void**)&Z2, nstate * 8, st));
-  ALZ_CUDA(cudaMallocAsync((void**)&E, nenv * 8, st));
-  ALZ_CUDA(cudaMallocAsync((void**)&E2, nenv * 8, st));
-  ALZ_CUDA(cudaMallocAsync((void**)&RL, (size_t)C * 8, st));
-  ALZ_CUDA(cudaMemsetAsync(Z1, 0, nstate * 8, st));
-  ALZ_CUDA(cudaMemsetAsync(E, 0, nenv * 8, st));
-  {   // the lowpass's chunk transition R^L (float64), one 1 x 1 matrix per channel; pageable source: staged before return
-    const std::vector<double> rl((size_t)C, std::pow(ep.R, (double)L));
-    ALZ_CUDA(cudaMemcpyAsync(RL, rl.data(), (size_t)C * 8, cudaMemcpyHostToDevice, st));
-  }
-  int rc = chunk_transition(p, L, st, &m);
+  const int C = p->C;
+  const long long V = S * P;                       // V virtual streams
+  const size_t nstate = (size_t)p->state_doubles * V * C, nenv = (size_t)V * C;
   AlzTileArgs ta{};
   // y feeds only the (unused) output tensor map: x stands in, as in the sequential launch
   ta.x = x; ta.y = const_cast<float*>(x); ta.S = V; ta.T = L; ta.xs = xs; ta.ys = xs; ta.ysS = (long long)C * xs; ta.C = C;
   ta.Stot = V;
   ta.vec_in = ta.vec_out = 1;
   ta.vP = (int)P;
-  if (rc == ALZ_OK) {
-    ta.exp = 2;                                    // pass 1: the plain bank kernel without tile stores
-    rc = apply_launch(p, ta, Z1, V * C, st, nullptr, 0);
-    ta.exp = 0;
+  StreamScratch<double> zero(st), init(st), E(st), E2(st), RL(st);
+  int rc = chunk_states(p, ta, state, sstride, P, L, st, zero, init);     // pass 1 and the bank-state scan
+  if (rc != ALZ_OK) return rc;
+  ALZ_CUDA(E.alloc(nenv));
+  ALZ_CUDA(E2.alloc(nenv));
+  ALZ_CUDA(RL.alloc(C));
+  ALZ_CUDA(cudaMemsetAsync(E.ptr, 0, nenv * 8, st));
+  {   // the lowpass's chunk transition R^L (float64), one 1 x 1 matrix per channel; pageable source: staged before return
+    const std::vector<double> rl((size_t)C, std::pow(ep.R, (double)L));
+    ALZ_CUDA(cudaMemcpyAsync(RL.ptr, rl.data(), (size_t)C * 8, cudaMemcpyHostToDevice, st));
   }
-  if (rc == ALZ_OK) {
-    alz_chunk_scan_kernel<<<dim3((unsigned)C, (unsigned)S), 32, 0, st>>>(Z1, Z2, m->M, state, sstride, sstride / C, d, C, S, P);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) rc = fail(ALZ_ERR_CUDA, "chunk scan launch failed: %s", cudaGetErrorString(e));
-  }
-  if (m) chunk_release(p, m);
-  if (rc == ALZ_OK) {
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    ALZ_CUDA(cudaMemcpyAsync(Z1, Z2, nstate * 8, cudaMemcpyDeviceToDevice, st));   // pass 2 overwrites Z2; pass 3 needs it
-    ta.state = Z2; ta.sstride = V * C;
-    ta.env_out = env; ta.env_es = es; ta.env_state = E; ta.env_g = ep.g; ta.env_R = ep.R; ta.env_decim = ep.decim;
-    ta.env_mode = ep.mode; ta.env_phase = ep.phase;
-    ta.env_store = 0;                              // pass 2: only the final lowpass states
-    rc = envelope_launch(p, ta, st);
-  }
-  if (rc == ALZ_OK) {
-    alz_chunk_scan_kernel<<<dim3((unsigned)C, (unsigned)S), 32, 0, st>>>(E, E2, RL, env_state, nenv, sstride / C, 1, C, S, P);
-    ALZ_CUDA(cudaGetLastError());
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    ta.state = Z1;
-    ta.env_state = E2;
-    ta.env_store = 1;                              // pass 3: the output
-    rc = envelope_launch(p, ta, st);
-  }
-  cudaFreeAsync(Z1, st); cudaFreeAsync(Z2, st); cudaFreeAsync(E, st); cudaFreeAsync(E2, st); cudaFreeAsync(RL, st);
-  if (rc == ALZ_OK && T > Tmain) {                 // left-over samples of all streams: the same decision again
-    EnvParams tail = ep;
-    tail.phase = (int)((ep.phase + Tmain) % ep.decim);
-    rc = envelope_impl(p, x + Tmain, env + (ep.phase + Tmain) / ep.decim, state, env_state, sstride, S, T - Tmain, xs, es, tail, st);
-  }
-  return rc;
+  ALZ_CUDA(cudaMemcpyAsync(zero.ptr, init.ptr, nstate * 8, cudaMemcpyDeviceToDevice, st));   // pass 2 overwrites init; pass 3 needs it
+  ta.state = init.ptr; ta.sstride = V * C;
+  ta.env_out = env; ta.env_es = es; ta.env_state = E.ptr; ta.env_g = ep.g; ta.env_R = ep.R; ta.env_decim = ep.decim;
+  ta.env_mode = ep.mode; ta.env_phase = ep.phase;
+  ta.env_store = 0;                                // pass 2: only the final lowpass states
+  rc = envelope_launch(p, ta, st);
+  if (rc != ALZ_OK) return rc;
+  alz_chunk_scan_kernel<<<dim3((unsigned)C, (unsigned)S), 32, 0, st>>>(E.ptr, E2.ptr, RL.ptr, env_state, nenv, sstride / C, 1, C, S, P);
+  ALZ_CUDA(cudaGetLastError());
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  ta.state = zero.ptr;
+  ta.env_state = E2.ptr;
+  ta.env_store = 1;                                // pass 3: the output
+  return envelope_launch(p, ta, st);
 }
 
 // One implementation for every envelope entry.  state: [slot][sstride] bank states; env_state: [C][sstride / C] lowpass
 // states (stream-fastest, like the bank's); env rows [S][C], stride es, (phase + T) / decim values each.  T > 0.
 static int envelope_impl(const alz_plan* p, const float* x, float* env, double* state, double* env_state, long long sstride,
-                         long long S, long long T, long long xs, long long es, const EnvParams& ep, cudaStream_t st) {
+                         long long S, long long T, long long xs, long long es, EnvParams ep, cudaStream_t st) {
   if (((uintptr_t)x & 15) || (xs & 3) || env_int("ALZ_NO_TMA", 0))
     return fail(ALZ_ERR_UNSUPPORTED, "envelope consumer needs 16-byte aligned x rows");
   long long P = 0, L = 0;
-  if (chunk_geometry(p, S, T, 3, &P, &L)) return envelope_chunked(p, x, env, state, env_state, sstride, S, T, xs, es, ep, P, L, st);
+  while (chunk_geometry(p, S, T, 3, &P, &L)) {
+    const int rc = envelope_chunked(p, x, env, state, env_state, sstride, S, xs, es, ep, P, L, st);
+    if (rc != ALZ_OK || T == P * L) return rc;
+    // left-over samples of all streams: the same decision again
+    env += (ep.phase + P * L) / ep.decim;
+    ep.phase = (int)((ep.phase + P * L) % ep.decim);
+    x += P * L;
+    T -= P * L;
+  }
   AlzTileArgs ta{};
   // y only feeds the output tensor map, which the envelope consumer never uses; it must be 16-byte aligned for the map to
   // be encoded, and env need not be (a block of a longer envelope row starts anywhere), so x, which must be, stands in.
@@ -1243,54 +1322,53 @@ static int envelope_impl(const alz_plan* p, const float* x, float* env, double* 
 }
 
 // whole: the block must hold whole decimation windows (the entries without a phase)
-static int envelope_check(const alz_plan* p, int64_t S, int64_t T, int64_t xs, int64_t es, int32_t decim, int32_t phase,
-                          int32_t mode, bool whole) {
+static int envelope_check(const alz_plan* p, int64_t S, int64_t T, int64_t xs, int64_t es, const EnvParams& ep, bool whole) {
   if (!p) return fail(ALZ_ERR_INVALID, "plan is null");
   if (p->device < 0) return fail(ALZ_ERR_CUDA, "design-only plan: no device");
-  if (S < 0 || T < 0 || decim < 1 || mode < 0 || mode > 2 || phase < 0 || phase >= decim) return fail(ALZ_ERR_INVALID, "bad argument");
-  if (whole && T % decim) return fail(ALZ_ERR_INVALID, "n_samples must be a multiple of the decimation factor");
-  if (xs < T || es < (phase + T) / decim) return fail(ALZ_ERR_INVALID, "row stride shorter than the row");
+  if (S < 0 || T < 0 || ep.decim < 1 || ep.mode < 0 || ep.mode > 2 || ep.phase < 0 || ep.phase >= ep.decim)
+    return fail(ALZ_ERR_INVALID, "bad argument");
+  if (whole && T % ep.decim) return fail(ALZ_ERR_INVALID, "n_samples must be a multiple of the decimation factor");
+  if (xs < T || es < (ep.phase + T) / ep.decim) return fail(ALZ_ERR_INVALID, "row stride shorter than the row");
   if (p->kind != ALZ_KIND_BIQUAD || p->K != 4 || p->C * ALZ_COEF_STRIDE(4, p->NB0) <= 512 || S > 65535ll * 32)
     return fail(ALZ_ERR_UNSUPPORTED, "the envelope consumer is built for the gammatone banks (4 sections per channel)");
   return ALZ_OK;
 }
 
 static int envelope_device(const alz_plan* p, const float* x, float* env, double* state, double* env_state, int64_t S,
-                           int64_t T, int64_t xs, int64_t es, const EnvParams& ep, void* cuda_stream) {
+                           int64_t T, int64_t xs, int64_t es, const EnvParams& ep, bool whole, void* cuda_stream) {
+  const int chk = envelope_check(p, S, T, xs, es, ep, whole);
+  if (chk != ALZ_OK) return chk;
   if (S == 0 || T == 0) return ALZ_OK;
   if (!x || !state || !env_state || (!env && (ep.phase + T) / ep.decim > 0)) return fail(ALZ_ERR_INVALID, "null buffer");
-  int cur = -1;
-  ALZ_CUDA(cudaGetDevice(&cur));
-  if (cur != p->device) ALZ_CUDA(cudaSetDevice(p->device));
-  const int rc = envelope_impl(p, x, env, state, env_state, (long long)S * p->C, S, T, xs, es, ep, (cudaStream_t)cuda_stream);
-  if (cur != p->device) cudaSetDevice(cur);
-  return rc;
+  DeviceScope dev(p->device);
+  ALZ_CUDA(dev.status);
+  return envelope_impl(p, x, env, state, env_state, (long long)S * p->C, S, T, xs, es, ep, (cudaStream_t)cuda_stream);
 }
 
 int32_t alz_apply_envelope_f32(const alz_plan* p, const float* x, float* env, double* state, double* env_state, int64_t S,
                                int64_t T, int64_t xs, int64_t es, int32_t decim, int32_t mode, double g, double R,
                                void* cuda_stream) {
-  const int chk = envelope_check(p, S, T, xs, es, decim, 0, mode, true);
-  if (chk != ALZ_OK) return chk;
-  return envelope_device(p, x, env, state, env_state, S, T, xs, es, EnvParams{decim, 0, mode, g, R}, cuda_stream);
+  return envelope_device(p, x, env, state, env_state, S, T, xs, es, EnvParams{decim, 0, mode, g, R}, true, cuda_stream);
 }
 
 int32_t alz_apply_envelope_f32_ex(const alz_plan* p, const float* x, float* env, double* state, double* env_state, int64_t S,
                                   int64_t T, int64_t xs, int64_t es, int32_t decim, int32_t phase, int32_t mode, double g,
                                   double R, void* cuda_stream) {
-  const int chk = envelope_check(p, S, T, xs, es, decim, phase, mode, false);
-  if (chk != ALZ_OK) return chk;
-  return envelope_device(p, x, env, state, env_state, S, T, xs, es, EnvParams{decim, phase, mode, g, R}, cuda_stream);
+  return envelope_device(p, x, env, state, env_state, S, T, xs, es, EnvParams{decim, phase, mode, g, R}, false, cuda_stream);
 }
 
 // Host buffers: chunks of whole streams through the plan's staging pipeline.  state / env_state: device, NULL = zero and
 // discarded (per-chunk staging states when both are NULL).
-static int envelope_host(alz_plan* p, const float* xh, float* eh, double* state, double* env_state, int64_t S, int64_t T,
-                         int64_t xs, int64_t es, const EnvParams& ep) {
+static int envelope_host(const alz_plan* cp, const float* xh, float* eh, double* state, double* env_state, int64_t S, int64_t T,
+                         int64_t xs, int64_t es, const EnvParams& ep, bool whole) {
+  const int chk = envelope_check(cp, S, T, xs, es, ep, whole);
+  if (chk != ALZ_OK) return chk;
+  alz_plan* p = const_cast<alz_plan*>(cp);
   if (S == 0 || T == 0) return ALZ_OK;
   if (!xh || (!eh && (ep.phase + T) / ep.decim > 0)) return fail(ALZ_ERR_INVALID, "null buffer");
   std::lock_guard<std::mutex> lock(p->host_mu);
-  ALZ_CUDA(cudaSetDevice(p->device));
+  DeviceScope dev(p->device);
+  ALZ_CUDA(dev.status);
   const int decim = ep.decim;
   const long long C = p->C, Td = (ep.phase + T) / decim, Tp = (T + 3) & ~3LL, Tdp = (Td + 3) & ~3LL;
   // chunks of whole streams: <= 64 MiB of input per chunk (the output is decim times smaller than the bank's)
@@ -1298,46 +1376,24 @@ static int envelope_host(alz_plan* p, const float* xh, float* eh, double* state,
   if (Sc > S) Sc = S;
   AlzHostPipe& hp = p->pipe;
   const int NB = AlzHostPipe::NBUF;
-  if (!hp.ready) {
-    for (int i = 0; i < NB; ++i) {
-      ALZ_CUDA(cudaStreamCreateWithFlags(&hp.stream[i], cudaStreamNonBlocking));
-      ALZ_CUDA(cudaEventCreateWithFlags(&hp.done[i], cudaEventDisableTiming));
-    }
-    hp.ready = true;
-  }
-  // staging buffers are kept in the plan between calls (grown on demand), as in alz_apply_f32_host
-  auto grow = [&](auto** bufs, size_t& have, size_t need) -> int {
-    if (have >= need) return ALZ_OK;
-    for (int i = 0; i < NB; ++i) {
-      ALZ_CUDA(cudaStreamSynchronize(hp.stream[i]));
-      cudaFree(bufs[i]);
-      bufs[i] = nullptr;
-    }
-    have = 0;
-    for (int i = 0; i < NB; ++i) ALZ_CUDA(cudaMalloc((void**)&bufs[i], need));
-    have = need;
-    return ALZ_OK;
-  };
   // Given states are indexed for all S streams ([slot][S * C], [C][S]).  When only one of the two is given, the other
   // gets a zeroed buffer of the same layout for this call.
-  double* own = nullptr;
+  DeviceBuffer own(nullptr, cudaFree);
   if ((state != nullptr) != (env_state != nullptr)) {
     const size_t bytes = (size_t)(state ? 1 : p->state_doubles) * S * C * 8;
-    ALZ_CUDA(cudaMalloc((void**)&own, bytes));
-    ALZ_CUDA(cudaMemset(own, 0, bytes));
-    (state ? env_state : state) = own;
+    double* buf = nullptr;
+    ALZ_CUDA(cudaMalloc((void**)&buf, bytes));
+    own.reset(buf);
+    ALZ_CUDA(cudaMemset(buf, 0, bytes));
+    (state ? env_state : state) = buf;
   }
   const bool given = state != nullptr;
-  // Ordering contract (include/alz_b200.h): given states must be complete, or produced by work on the legacy default
-  // stream: the private pipeline streams are ordered after it.
-  if (given) {
-    ALZ_CUDA(cudaEventRecord(hp.done[0], cudaStreamLegacy));
-    for (int k = 0; k < NB; ++k) ALZ_CUDA(cudaStreamWaitEvent(hp.stream[k], hp.done[0], 0));
-  }
-  int rc = grow(hp.dx, hp.dx_bytes, (size_t)Sc * Tp * 4);
-  if (rc == ALZ_OK) rc = grow(hp.dy, hp.dy_bytes, (size_t)Sc * C * Tdp * 4);
-  if (rc == ALZ_OK && !given) rc = grow(hp.dst, hp.dst_bytes, (size_t)p->state_doubles * Sc * C * 8);
-  if (rc == ALZ_OK && !given) rc = grow(hp.des, hp.des_bytes, (size_t)Sc * C * 8);
+  int rc = pipe_open(hp, given);
+  if (rc != ALZ_OK) return rc;
+  rc = pipe_grow(hp, hp.dx, hp.dx_bytes, (size_t)Sc * Tp * 4);
+  if (rc == ALZ_OK) rc = pipe_grow(hp, hp.dy, hp.dy_bytes, (size_t)Sc * C * Tdp * 4);
+  if (rc == ALZ_OK && !given) rc = pipe_grow(hp, hp.dst, hp.dst_bytes, (size_t)p->state_doubles * Sc * C * 8);
+  if (rc == ALZ_OK && !given) rc = pipe_grow(hp, hp.des, hp.des_bytes, (size_t)Sc * C * 8);
   int i = 0;
   for (long long s0 = 0; s0 < S && rc == ALZ_OK; s0 += Sc, ++i) {
     const long long n = std::min<long long>(Sc, S - s0);
@@ -1359,55 +1415,37 @@ static int envelope_host(alz_plan* p, const float* xh, float* eh, double* state,
       if (e != cudaSuccess) { rc = fail(ALZ_ERR_CUDA, "D2H copy failed: %s", cudaGetErrorString(e)); break; }
     }
   }
-  for (int k = 0; k < NB; ++k) {
-    cudaError_t e = cudaStreamSynchronize(hp.stream[k]);
-    if (e != cudaSuccess && rc == ALZ_OK) rc = fail(ALZ_ERR_CUDA, "pipeline failed: %s", cudaGetErrorString(e));
-  }
-  cudaFree(own);
-  return rc;
+  return pipe_finish(hp, rc);
 }
 
-int32_t alz_apply_envelope_f32_host(const alz_plan* cp, const float* xh, float* eh, int64_t S, int64_t T, int64_t xs, int64_t es,
+int32_t alz_apply_envelope_f32_host(const alz_plan* p, const float* xh, float* eh, int64_t S, int64_t T, int64_t xs, int64_t es,
                                     int32_t decim, int32_t mode, double g, double R) {
-  alz_plan* p = const_cast<alz_plan*>(cp);
-  const int chk = envelope_check(p, S, T, xs, es, decim, 0, mode, true);
-  if (chk != ALZ_OK) return chk;
-  return envelope_host(p, xh, eh, nullptr, nullptr, S, T, xs, es, EnvParams{decim, 0, mode, g, R});
+  return envelope_host(p, xh, eh, nullptr, nullptr, S, T, xs, es, EnvParams{decim, 0, mode, g, R}, true);
 }
 
-int32_t alz_apply_envelope_f32_host_ex(const alz_plan* cp, const float* xh, float* eh, double* state, double* env_state,
+int32_t alz_apply_envelope_f32_host_ex(const alz_plan* p, const float* xh, float* eh, double* state, double* env_state,
                                        int64_t S, int64_t T, int64_t xs, int64_t es, int32_t decim, int32_t phase, int32_t mode,
                                        double g, double R) {
-  alz_plan* p = const_cast<alz_plan*>(cp);
-  const int chk = envelope_check(p, S, T, xs, es, decim, phase, mode, false);
-  if (chk != ALZ_OK) return chk;
-  return envelope_host(p, xh, eh, state, env_state, S, T, xs, es, EnvParams{decim, phase, mode, g, R});
+  return envelope_host(p, xh, eh, state, env_state, S, T, xs, es, EnvParams{decim, phase, mode, g, R}, false);
 }
 
 int32_t alz_apply_sum_f32(const alz_plan* p, const float* x, float* out, double* state, int64_t S, int64_t T,
                           int64_t xs, int64_t os, void* cuda_stream) {
-  if (!p) return fail(ALZ_ERR_INVALID, "plan is null");
-  if (p->device < 0) return fail(ALZ_ERR_CUDA, "design-only plan: no device");
-  if (S < 0 || T < 0) return fail(ALZ_ERR_INVALID, "negative size");
-  if (S == 0 || T == 0) return ALZ_OK;
-  if (!x || !out || !state) return fail(ALZ_ERR_INVALID, "null buffer");
-  if (xs < T || os < T) return fail(ALZ_ERR_INVALID, "row stride shorter than n_samples");
+  int rc;
+  if (!apply_check(p, true, S, T, x && out && state, xs, os, &rc)) return rc;
   if (p->kind != ALZ_KIND_BIQUAD || !p->parallel_sum || p->NB0 != 0 || p->monic != 0 || p->chunks.size() != 1)
     return fail(ALZ_ERR_UNSUPPORTED, "alz_apply_sum_f32 needs a biquad plan created with ALZ_PLAN_PARALLEL");
   if (S > 65535ll * 32) return fail(ALZ_ERR_UNSUPPORTED, "too many streams for one launch");
   CUtensorMap tmx, tmo;
   if (env_int("ALZ_NO_TMA", 0) || !make_map_2d(x, T, S, xs, &tmx) || !make_map_2d(out, T, S, os, &tmo))
     return fail(ALZ_ERR_UNSUPPORTED, "alz_apply_sum_f32 needs 16-byte aligned rows (use alz_apply_f32 + alz_sum_channels_f32)");
-  int cur = -1;
-  ALZ_CUDA(cudaGetDevice(&cur));
-  if (cur != p->device) ALZ_CUDA(cudaSetDevice(p->device));
+  DeviceScope dev(p->device);
+  ALZ_CUDA(dev.status);
   AlzTileArgs ta{};
   ta.x = x; ta.y = out; ta.S = S; ta.T = T; ta.xs = xs; ta.ys = os; ta.ysS = os; ta.C = p->C; ta.Stot = S;
   ta.state = state; ta.sstride = (long long)S * p->C;
   ta.vec_in = ta.vec_out = 1;
-  const int rc = alzi_launch_parallel(p, ta, tmx, tmo, (cudaStream_t)cuda_stream);
-  if (cur != p->device) cudaSetDevice(cur);
-  return rc;
+  return alzi_launch_parallel(p, ta, tmx, tmo, (cudaStream_t)cuda_stream);
 }
 
 int32_t alz_plan_taps(const alz_plan* p, int32_t* delay, int32_t* is_den, int32_t cap) {
@@ -1426,29 +1464,21 @@ int32_t alz_apply_tv_f32(const alz_plan* p, const float* x, float* y, double* st
   if (!p) return fail(ALZ_ERR_INVALID, "plan is null");
   if (p->kind != ALZ_KIND_GENERIC || p->C != 1 || p->window)
     return fail(ALZ_ERR_UNSUPPORTED, "time-varying coefficients need a single-channel generic plan (alz_plan_create_ex with ALZ_PLAN_FORCE_GENERIC)");
-  if (S < 0 || T < 0) return fail(ALZ_ERR_INVALID, "negative size");
-  if (S == 0 || T == 0) return ALZ_OK;
-  if (!x || !y || !state || !coef_dev) return fail(ALZ_ERR_INVALID, "null buffer");
-  if (xs < T || ys < T || coef_stride < T) return fail(ALZ_ERR_INVALID, "row stride shorter than n_samples");
-  int cur = -1;
-  ALZ_CUDA(cudaGetDevice(&cur));
-  if (cur != p->device) ALZ_CUDA(cudaSetDevice(p->device));
-  const int rc = apply_impl(p, x, y, state, (long long)S, S, T, xs, ys, (cudaStream_t)cuda_stream, coef_dev, coef_stride, 0);
-  if (cur != p->device) cudaSetDevice(cur);
-  return rc;
+  int rc;
+  if (!apply_check(p, false, S, T, x && y && state && coef_dev, xs, std::min(ys, coef_stride), &rc)) return rc;
+  DeviceScope dev(p->device);
+  ALZ_CUDA(dev.status);
+  return apply_impl(p, x, y, state, (long long)S, S, T, xs, ys, ys, (cudaStream_t)cuda_stream, coef_dev, coef_stride);
 }
 
 int32_t alz_apply_f32_host(const alz_plan* cp, const float* xh, float* yh, double* state, int64_t S, int64_t T,
                            int64_t xs, int64_t ys) {
   alz_plan* p = const_cast<alz_plan*>(cp);
-  if (!p) return fail(ALZ_ERR_INVALID, "plan is null");
-  if (p->device < 0) return fail(ALZ_ERR_CUDA, "design-only plan: no device");
-  if (S < 0 || T < 0) return fail(ALZ_ERR_INVALID, "negative size");
-  if (S == 0 || T == 0) return ALZ_OK;
-  if (!xh || !yh) return fail(ALZ_ERR_INVALID, "null buffer");
-  if (xs < T || ys < T) return fail(ALZ_ERR_INVALID, "row stride shorter than n_samples");
+  int rc;
+  if (!apply_check(p, true, S, T, xh && yh, xs, ys, &rc)) return rc;
   std::lock_guard<std::mutex> lock(p->host_mu);
-  ALZ_CUDA(cudaSetDevice(p->device));
+  DeviceScope dev(p->device);
+  ALZ_CUDA(dev.status);
   AlzHostPipe& hp = p->pipe;
   const long long C = p->C;
   const long long kChunkBytes = 128LL << 20;   // <= 128 MiB of output per staged chunk
@@ -1463,43 +1493,19 @@ int32_t alz_apply_f32_host(const alz_plan* cp, const float* xh, float* yh, doubl
   long long Sc = kChunkBytes / (C * Tp * 4);
   if (Sc < 1) Sc = 1;
   if (Sc > S) Sc = S;
-  const size_t need_x = (size_t)Sc * Tp * 4, need_y = (size_t)Sc * C * Tp * 4;
-  if (!hp.ready) {
-    for (int i = 0; i < AlzHostPipe::NBUF; ++i) {
-      ALZ_CUDA(cudaStreamCreateWithFlags(&hp.stream[i], cudaStreamNonBlocking));
-      ALZ_CUDA(cudaEventCreateWithFlags(&hp.done[i], cudaEventDisableTiming));
-    }
-    hp.ready = true;
-  }
-  // Ordering contract (include/alz_b200.h): a caller-supplied state must be complete, or produced by work on the
-  // legacy default stream (where torch launches by default): the private pipeline streams are ordered after it.
-  if (state) {
-    ALZ_CUDA(cudaEventRecord(hp.done[0], cudaStreamLegacy));
-    for (int i = 0; i < AlzHostPipe::NBUF; ++i) ALZ_CUDA(cudaStreamWaitEvent(hp.stream[i], hp.done[0], 0));
-  }
-  if (hp.dx_bytes < need_x || hp.dy_bytes < need_y) {
-    for (int i = 0; i < AlzHostPipe::NBUF; ++i) {
-      ALZ_CUDA(cudaStreamSynchronize(hp.stream[i]));
-      cudaFree(hp.dx[i]); hp.dx[i] = nullptr;
-      cudaFree(hp.dy[i]); hp.dy[i] = nullptr;
-    }
-    hp.dx_bytes = hp.dy_bytes = 0;
-    for (int i = 0; i < AlzHostPipe::NBUF; ++i) {
-      ALZ_CUDA(cudaMalloc(&hp.dx[i], need_x));
-      ALZ_CUDA(cudaMalloc(&hp.dy[i], need_y));
-    }
-    hp.dx_bytes = need_x;
-    hp.dy_bytes = need_y;
-  }
+  rc = pipe_open(hp, state != nullptr);
+  if (rc == ALZ_OK) rc = pipe_grow(hp, hp.dx, hp.dx_bytes, (size_t)Sc * Tp * 4);
+  if (rc == ALZ_OK) rc = pipe_grow(hp, hp.dy, hp.dy_bytes, (size_t)Sc * C * Tp * 4);
+  if (rc != ALZ_OK) return rc;
+  DeviceBuffer own(nullptr, cudaFree);   // zero initial state when none is given
   double* st_buf = state;
-  bool own_state = false;
   if (!st_buf) {
-    ALZ_CUDA(cudaMalloc(&st_buf, (size_t)p->state_doubles * S * C * sizeof(double)));
-    own_state = true;
-    ALZ_CUDA(cudaMemsetAsync(st_buf, 0, (size_t)p->state_doubles * S * C * sizeof(double), hp.stream[0]));
+    const size_t bytes = (size_t)p->state_doubles * S * C * sizeof(double);
+    ALZ_CUDA(cudaMalloc(&st_buf, bytes));
+    own.reset(st_buf);
+    ALZ_CUDA(cudaMemsetAsync(st_buf, 0, bytes, hp.stream[0]));
     ALZ_CUDA(cudaStreamSynchronize(hp.stream[0]));
   }
-  int rc = ALZ_OK;
   int i = 0;
   for (long long s0 = 0; s0 < S && rc == ALZ_OK; s0 += Sc) {
     const long long n = std::min<long long>(Sc, S - s0);
@@ -1511,7 +1517,7 @@ int32_t alz_apply_f32_host(const alz_plan* cp, const float* xh, float* yh, doubl
       if (prev) { cudaStreamWaitEvent(st, prev, 0); cudaEventDestroy(prev); prev = nullptr; }
       cudaError_t e = cudaMemcpy2DAsync(hp.dx[b], Tp * 4, xh + s0 * xs + t0, xs * 4, nt * 4, n, cudaMemcpyHostToDevice, st);
       if (e != cudaSuccess) { rc = fail(ALZ_ERR_CUDA, "H2D copy failed: %s", cudaGetErrorString(e)); break; }
-      rc = apply_plain(p, hp.dx[b], hp.dy[b], st_buf + s0, (long long)S * C, n, nt, Tp, Tp, st);
+      rc = apply_impl(p, hp.dx[b], hp.dy[b], st_buf + s0, (long long)S * C, n, nt, Tp, Tp, C * Tp, st);
       if (rc != ALZ_OK) break;
       if (t0 + Tc < T) {
         cudaEventCreateWithFlags(&prev, cudaEventDisableTiming);
@@ -1522,12 +1528,7 @@ int32_t alz_apply_f32_host(const alz_plan* cp, const float* xh, float* yh, doubl
     }
     if (prev) cudaEventDestroy(prev);
   }
-  for (int k = 0; k < AlzHostPipe::NBUF; ++k) {
-    cudaError_t e = cudaStreamSynchronize(hp.stream[k]);
-    if (e != cudaSuccess && rc == ALZ_OK) rc = fail(ALZ_ERR_CUDA, "pipeline failed: %s", cudaGetErrorString(e));
-  }
-  if (own_state) cudaFree(st_buf);
-  return rc;
+  return pipe_finish(hp, rc);
 }
 
 static __global__ void alz_sum_channels_kernel(const float* y, float* out, long long S, int C, long long T, long long ys,
@@ -1596,23 +1597,19 @@ int32_t alz_freq_response_f64(alz_plan* p, const double* w, double* out, int64_t
   if (n < 0) return fail(ALZ_ERR_INVALID, "negative size");
   if (n == 0) return ALZ_OK;
   if (!w || !out) return fail(ALZ_ERR_INVALID, "null buffer");
-  int cur = -1;
-  ALZ_CUDA(cudaGetDevice(&cur));
-  if (cur != p->device) ALZ_CUDA(cudaSetDevice(p->device));
+  DeviceScope dev(p->device);
+  ALZ_CUDA(dev.status);
   {
     std::lock_guard<std::mutex> lock(p->host_mu);
     if (!p->d_fr_desc) {
-      ALZ_CUDA(cudaMalloc(&p->d_fr_desc, p->fr_desc.size() * sizeof(int)));
-      ALZ_CUDA(cudaMalloc(&p->d_fr_coef, std::max<size_t>(1, p->fr_coef.size()) * sizeof(double)));
-      ALZ_CUDA(cudaMemcpy(p->d_fr_desc, p->fr_desc.data(), p->fr_desc.size() * sizeof(int), cudaMemcpyHostToDevice));
-      ALZ_CUDA(cudaMemcpy(p->d_fr_coef, p->fr_coef.data(), p->fr_coef.size() * sizeof(double), cudaMemcpyHostToDevice));
+      const int rc = upload_tables(p, {table(&p->d_fr_desc, p->fr_desc), table(&p->d_fr_coef, p->fr_coef)});
+      if (rc != ALZ_OK) return rc;
     }
   }
   alz_freq_response_kernel<<<dim3((unsigned)((n + 127) / 128), (unsigned)p->C), 128, 0, (cudaStream_t)cuda_stream>>>(
       p->d_fr_coef, p->d_fr_desc, p->C, p->fr_K, w, n, out);
   ALZ_CUDA(cudaGetLastError());
   g_launches.fetch_add(1, std::memory_order_relaxed);
-  if (cur != p->device) cudaSetDevice(cur);
   return ALZ_OK;
 }
 

@@ -91,7 +91,9 @@ int32_t alz_abi_version(void);
 int32_t alz_device_count(void);
 
 /* Make `device` the current CUDA device of the calling thread for this library
- * (plans are created on the current device; apply calls use the plan's device). */
+ * (plans are created on the current device; apply calls use the plan's device).  Every call that
+ * takes a plan, the host-buffer entries and alz_state_init included, works on the plan's device and
+ * returns with the caller's current device unchanged, on success and on error. */
 int32_t alz_set_device(int32_t device);
 
 /*
