@@ -21,6 +21,11 @@ The three analysis libraries also include ``csrc_common/alz_common.h``.
 overlap-add sums reproduce AudioLazy's bit for bit), which also includes ``csrc_common/alz_common.h``.  It sits next to
 :data:`LIBRARIES` rather than in it because the test of the library bindings pins that dict to the four libraries
 above; folding it in means extending that test's table, a follow-up.
+
+:data:`RESAMPLE` is a sixth library, built last and kept out of :data:`LIBRARIES` for the same reason:
+``libalz_b200_resample.so``, the Lagrange resampling library (``csrc_resample/*.cu`` behind
+``include/alz_b200_resample.h``, compiled with ``-fmad=false``: its weights and compensated sums reproduce AudioLazy's
+bit for bit), which also includes ``csrc_common/alz_common.h``.
 """
 from __future__ import annotations
 
@@ -76,12 +81,16 @@ LIBRARIES = {lib.name: lib for lib in (
 )}
 #: the short-time Fourier library (see the module docstring for why it is not in :data:`LIBRARIES`)
 STFT = Library("stft", "libalz_b200_stft.so", "csrc_stft", "alz_b200_stft.h", ("-fmad=false",), _COMMON)
+#: the resampling library (outside :data:`LIBRARIES` for the same reason as :data:`STFT`)
+RESAMPLE = Library("resample", "libalz_b200_resample.so", "csrc_resample", "alz_b200_resample.h", ("-fmad=false",),
+                   _COMMON)
 #: the filter library (``_capi`` loads it from here unless ``ALZ_B200_LIB`` names another file)
 LIB_PATH = LIBRARIES["filters"].path
 AMDF_LIB_PATH = LIBRARIES["amdf"].path
 ZCROSS_LIB_PATH = LIBRARIES["zcross"].path
 LPC_LIB_PATH = LIBRARIES["lpc"].path
 STFT_LIB_PATH = STFT.path
+RESAMPLE_LIB_PATH = RESAMPLE.path
 
 
 def is_stale(lib: Library) -> bool:
@@ -98,8 +107,8 @@ def find_nvcc():
 
 
 def build_native(force: bool = False, verbose: bool = False) -> list:
-  """Build every library of :data:`LIBRARIES`, then :data:`STFT`; returns their paths."""
-  return [build_library(lib, force=force, verbose=verbose) for lib in list(LIBRARIES.values()) + [STFT]]
+  """Build every library of :data:`LIBRARIES`, then :data:`STFT` and :data:`RESAMPLE`; returns their paths."""
+  return [build_library(lib, force=force, verbose=verbose) for lib in list(LIBRARIES.values()) + [STFT, RESAMPLE]]
 
 
 def build_library(lib: Library, force: bool = False, verbose: bool = False) -> str:

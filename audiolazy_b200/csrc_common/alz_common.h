@@ -1,4 +1,4 @@
-// alz_common.h -- host plumbing and block arithmetic shared by the AMDF, zero-crossing and LPC libraries.
+// alz_common.h -- host plumbing, block arithmetic and the compensated sum shared by the analysis libraries.
 //
 // Everything here is in an unnamed namespace: each library's unit gets its own copy, so the message a library's
 // *_last_error() returns is that library's own last failure.
@@ -52,5 +52,19 @@ inline long long emitted_blocks(long long consumed, long long n_samples, int siz
   if (final && consumed + n_samples - kp * hop > (size > hop ? size - hop : 0)) ++n;
   return n;
 }
+
+// Running compensated sum: CPython 3.12's sum() of floats (Neumaier), started from 0.0 and compensated from the first
+// term on, which gives the same value (see alz_lpc.cu).  The units that use it are compiled with -fmad=false.
+struct Psum {
+  double f = 0.0, c = 0.0;
+  __device__ __forceinline__ void add(double x) {
+    const double t = __dadd_rn(f, x);
+    const bool big = fabs(f) >= fabs(x);
+    const double hi = big ? f : x, lo = big ? x : f;
+    c = __dadd_rn(c, __dadd_rn(__dsub_rn(hi, t), lo));
+    f = t;
+  }
+  __device__ __forceinline__ double value() const { return (c != 0.0 && isfinite(c)) ? __dadd_rn(f, c) : f; }
+};
 
 }  // namespace

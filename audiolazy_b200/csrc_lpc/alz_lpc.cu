@@ -55,19 +55,6 @@ struct LpcArgs {
 
 long long state_stride(int size) { return (16 + 4 * (long long)size + 7) / 8 * 8; }
 
-// Running compensated sum (the header's psum).
-struct Psum {
-  double f = 0.0, c = 0.0;
-  __device__ __forceinline__ void add(double x) {
-    const double t = __dadd_rn(f, x);
-    const bool big = fabs(f) >= fabs(x);
-    const double hi = big ? f : x, lo = big ? x : f;
-    c = __dadd_rn(c, __dadd_rn(__dsub_rn(hi, t), lo));
-    f = t;
-  }
-  __device__ __forceinline__ double value() const { return (c != 0.0 && isfinite(c)) ? __dadd_rn(f, c) : f; }
-};
-
 int frames_per_cta(int ncell, int size) {
   int fpc = kThreadsAcorr / ncell;
   const int by_smem = kSmemBudget / (8 * (size + 1));

@@ -19,7 +19,7 @@ Coefficients may be :class:`~audiolazy_b200.stream.Stream` instances (time-varyi
 filters): as in the reference they are kept whatever their values, compared by identity,
 tee-copied by :meth:`Poly.copy`, and fanned out with ``thub`` when a product or a division
 uses them more than once (``lazy_poly.py:388-402, 449-462``). ``lagrange`` and ``resample``
-are out of scope.
+(``lazy_poly.py:493-603``) live in :mod:`audiolazy_b200.resampling`.
 """
 from __future__ import annotations
 
