@@ -3,7 +3,7 @@
 ``nvcc`` cross-compiles for sm_90a (H100) without a GPU; the built ``.so`` files are git-ignored
 but travel to the GPU box with the repository snapshot.
 
-:data:`LIBRARIES` lists the four libraries.  Each one is the ``.cu`` units of its source directory, compiled in
+:data:`LIBRARIES` lists the six libraries.  Each one is the ``.cu`` units of its source directory, compiled in
 parallel into ``_native/obj/<name>/`` (only the units that changed) and linked into one shared library:
 
 * ``libalz_b200.so``, the filter library: ``csrc/*.cu`` behind ``include/alz_b200.h`` (the C ABI plus one unit of
@@ -13,19 +13,13 @@ parallel into ``_native/obj/<name>/`` (only the units that changed) and linked i
 * ``libalz_b200_zcross.so``, the zero-crossing library: ``csrc_zcross/*.cu`` behind ``include/alz_b200_zcross.h``.
 * ``libalz_b200_lpc.so``, the frame-wise LPC library: ``csrc_lpc/*.cu`` behind ``include/alz_b200_lpc.h``, compiled
   with ``-fmad=false`` (its float64 sums reproduce AudioLazy's bit for bit).
+* ``libalz_b200_stft.so``, the short-time Fourier library: ``csrc_stft/*.cu`` behind ``include/alz_b200_stft.h``,
+  compiled with ``-fmad=false`` (its window products and overlap-add sums reproduce AudioLazy's bit for bit).
+* ``libalz_b200_resample.so``, the Lagrange resampling library: ``csrc_resample/*.cu`` behind
+  ``include/alz_b200_resample.h``, compiled with ``-fmad=false`` (its weights and compensated sums reproduce
+  AudioLazy's bit for bit).
 
-The three analysis libraries also include ``csrc_common/alz_common.h``.
-
-:data:`STFT` is a fifth library, built after those four: ``libalz_b200_stft.so``, the short-time Fourier library
-(``csrc_stft/*.cu`` behind ``include/alz_b200_stft.h``, compiled with ``-fmad=false``: its window products and
-overlap-add sums reproduce AudioLazy's bit for bit), which also includes ``csrc_common/alz_common.h``.  It sits next to
-:data:`LIBRARIES` rather than in it because the test of the library bindings pins that dict to the four libraries
-above; folding it in means extending that test's table, a follow-up.
-
-:data:`RESAMPLE` is a sixth library, built last and kept out of :data:`LIBRARIES` for the same reason:
-``libalz_b200_resample.so``, the Lagrange resampling library (``csrc_resample/*.cu`` behind
-``include/alz_b200_resample.h``, compiled with ``-fmad=false``: its weights and compensated sums reproduce AudioLazy's
-bit for bit), which also includes ``csrc_common/alz_common.h``.
+The five analysis libraries also include ``csrc_common/alz_common.h``.
 """
 from __future__ import annotations
 
@@ -78,19 +72,11 @@ LIBRARIES = {lib.name: lib for lib in (
   Library("amdf", "libalz_b200_amdf.so", "csrc_amdf", "alz_b200_amdf.h", ("-fmad=false",), _COMMON),
   Library("zcross", "libalz_b200_zcross.so", "csrc_zcross", "alz_b200_zcross.h", (), _COMMON),
   Library("lpc", "libalz_b200_lpc.so", "csrc_lpc", "alz_b200_lpc.h", ("-fmad=false",), _COMMON),
+  Library("stft", "libalz_b200_stft.so", "csrc_stft", "alz_b200_stft.h", ("-fmad=false",), _COMMON),
+  Library("resample", "libalz_b200_resample.so", "csrc_resample", "alz_b200_resample.h", ("-fmad=false",), _COMMON),
 )}
-#: the short-time Fourier library (see the module docstring for why it is not in :data:`LIBRARIES`)
-STFT = Library("stft", "libalz_b200_stft.so", "csrc_stft", "alz_b200_stft.h", ("-fmad=false",), _COMMON)
-#: the resampling library (outside :data:`LIBRARIES` for the same reason as :data:`STFT`)
-RESAMPLE = Library("resample", "libalz_b200_resample.so", "csrc_resample", "alz_b200_resample.h", ("-fmad=false",),
-                   _COMMON)
 #: the filter library (``_capi`` loads it from here unless ``ALZ_B200_LIB`` names another file)
 LIB_PATH = LIBRARIES["filters"].path
-AMDF_LIB_PATH = LIBRARIES["amdf"].path
-ZCROSS_LIB_PATH = LIBRARIES["zcross"].path
-LPC_LIB_PATH = LIBRARIES["lpc"].path
-STFT_LIB_PATH = STFT.path
-RESAMPLE_LIB_PATH = RESAMPLE.path
 
 
 def is_stale(lib: Library) -> bool:
@@ -107,8 +93,8 @@ def find_nvcc():
 
 
 def build_native(force: bool = False, verbose: bool = False) -> list:
-  """Build every library of :data:`LIBRARIES`, then :data:`STFT` and :data:`RESAMPLE`; returns their paths."""
-  return [build_library(lib, force=force, verbose=verbose) for lib in list(LIBRARIES.values()) + [STFT, RESAMPLE]]
+  """Build every library of :data:`LIBRARIES`; returns their paths."""
+  return [build_library(lib, force=force, verbose=verbose) for lib in LIBRARIES.values()]
 
 
 def build_library(lib: Library, force: bool = False, verbose: bool = False) -> str:

@@ -21,7 +21,7 @@ __all__ = ["amdf", "AmdfBank", "AmdfState"]
 PLAN_SEQUENTIAL = 8
 
 _i32, _i64, _f64, _vp = ctypes.c_int32, ctypes.c_int64, ctypes.c_double, ctypes.c_void_p
-LIB = _capi.NativeLib(_build.AMDF_LIB_PATH, "AMDF", {
+LIB = _capi.NativeLib(_build.LIBRARIES["amdf"].path, "AMDF", {
   "alz_amdf_last_error": (ctypes.c_char_p, []),
   "alz_amdf_plan_create": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, ctypes.POINTER(_vp)]),
   "alz_amdf_plan_destroy": (None, [_vp]),

@@ -20,7 +20,7 @@ from .stream import Stream
 __all__ = ["zcross", "Zcross", "ZcrossState"]
 
 _i32, _i64, _f64, _vp = ctypes.c_int32, ctypes.c_int64, ctypes.c_double, ctypes.c_void_p
-LIB = _capi.NativeLib(_build.ZCROSS_LIB_PATH, "zero-crossing", {
+LIB = _capi.NativeLib(_build.LIBRARIES["zcross"].path, "zero-crossing", {
   "alz_zcross_last_error": (ctypes.c_char_p, []),
   "alz_zcross_state_bytes": (_i64, [_i64, _i32, _i32]),
   "alz_zcross_state_init": (_i32, [_vp, _i64, _f64, _i32, _i32, _vp]),

@@ -21,8 +21,6 @@
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
-#include <mutex>
-#include <set>
 #include <vector>
 
 namespace {
@@ -179,19 +177,10 @@ __global__ void __launch_bounds__(kThreads) alz_amdf_kernel(const __grid_constan
 }
 
 // After a block: the history becomes the last H samples of (history, block), the running means those the last chunk
-// left, and the count advances.  In place, ascending: new[i] reads old[i + T], which no earlier chunk has written.
+// left, and the count advances.
 __global__ void __launch_bounds__(256) alz_amdf_commit_kernel(const __grid_constant__ AmdfArgs a) {
   double* st = a.state + (long long)blockIdx.x * a.sstride;
-  double* hist = st + 2;
-  const float* xr = a.x + (long long)blockIdx.x * a.xs;
-  for (long long i0 = 0; i0 < a.H; i0 += blockDim.x) {
-    const long long i = i0 + threadIdx.x, p = a.T - a.H + i;
-    double v = 0.0;
-    if (i < a.H) v = p >= 0 ? (double)xr[p] : hist[i + a.T];
-    __syncthreads();
-    if (i < a.H) hist[i] = v;
-    __syncthreads();
-  }
+  shift_history(st + 2, a.H, a.x + (long long)blockIdx.x * a.xs, a.T);
   for (int l = threadIdx.x; l < a.L; l += blockDim.x) st[2 + a.H + l] = st[2 + a.H + a.L + l];
   if (threadIdx.x == 0) st[0] = st[0] + (double)a.T;
 }
@@ -213,22 +202,6 @@ long long chunks(const AmdfPlan* p, long long S, long long T) {
   long long P = std::min(T / min_len, (2 * slots + warps - 1) / warps);
   P = std::min(P, (long long)0x7fffffff / (S * p->n_groups));
   return P < 2 ? 1 : P;
-}
-
-// The kernel's dynamic shared-memory limit is an attribute of the function in the device's context, shared by every
-// plan: it is raised once per device to the opt-in maximum (each launch asks for its own plan's size), never set to one
-// plan's size, which would make launches of a plan with a longer delay fail after a later plan with a shorter one.
-cudaError_t allow_max_smem(int device, int max_smem) {
-  static std::mutex mu;
-  static std::set<int> done;
-  std::lock_guard<std::mutex> lock(mu);
-  if (done.count(device)) return cudaSuccess;
-  cudaFuncAttributes fa;
-  cudaError_t e = cudaFuncGetAttributes(&fa, alz_amdf_kernel);
-  if (e == cudaSuccess)
-    e = cudaFuncSetAttribute(alz_amdf_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem - (int)fa.sharedSizeBytes);
-  if (e == cudaSuccess) done.insert(device);
-  return e;
 }
 
 }  // namespace
@@ -309,7 +282,7 @@ int32_t alz_amdf_plan_create(const int32_t* n_taps, const int32_t* delays, const
       table[(size_t)g * kThreads + i].group_mixed = mixed;
     }
   }
-  e = allow_max_smem(p->device, max_smem);
+  e = allow_dynamic_smem((const void*)alz_amdf_kernel, p->smem);
   if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&p->ctas_per_sm, alz_amdf_kernel, kThreads, p->smem);
   if (e == cudaSuccess) e = cudaMalloc((void**)&p->d_lags, table.size() * sizeof(AmdfLag));
   if (e == cudaSuccess) e = cudaMemcpy(p->d_lags, table.data(), table.size() * sizeof(AmdfLag), cudaMemcpyHostToDevice);

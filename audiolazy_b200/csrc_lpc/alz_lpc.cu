@@ -53,8 +53,6 @@ struct LpcArgs {
   int ncell;            // statistics per frame: order + 1 lags, or the (order + 1)(order + 2) / 2 cells of a triangle
 };
 
-long long state_stride(int size) { return (16 + 4 * (long long)size + 7) / 8 * 8; }
-
 int frames_per_cta(int ncell, int size) {
   int fpc = kThreadsAcorr / ncell;
   const int by_smem = kSmemBudget / (8 * (size + 1));
@@ -91,23 +89,14 @@ __global__ void __launch_bounds__(kMaxFramesPerCta * 32) alz_lpc_kernel(const __
   extern __shared__ double s_b[];              // [fpc][size + 1]
   const long long s = blockIdx.x / a.blocks_per_stream;
   const long long i0 = (long long)(blockIdx.x % a.blocks_per_stream) * a.fpc;
-  const unsigned char* st = a.state + s * a.sstride;
-  const long long C = *reinterpret_cast<const long long*>(st);
-  const float* tail = reinterpret_cast<const float*>(st + 16);    // samples [C - size, C)
-  const float* xr = a.x + s * a.xs;
-  const long long ka = first_open_block(C, a.size, a.hop);
+  const FramedSamples in = framed_samples(a.state + s * a.sstride, a.x + s * a.xs, a.T, a.size);
+  const long long ka = first_open_block(in.C, a.size, a.hop);
   const int size = a.size, ld = size + 1;
   const int nf = (int)(a.F - i0 < a.fpc ? a.F - i0 : a.fpc);
 
   for (int e = threadIdx.x; e < nf * size; e += blockDim.x) {
     const int f = e / size, n = e - f * size;
-    const long long g = (ka + i0 + f) * a.hop + n;                  // stream sample index
-    float v = 0.f;
-    if (g < C) {
-      v = tail[g - (C - size)];
-    } else if (g < C + a.T) {
-      v = xr[g - C];
-    }
+    const float v = in((ka + i0 + f) * a.hop + n);
     s_b[f * ld + n] = a.w ? __dmul_rn((double)v, a.w[n]) : (double)v;
   }
   __syncthreads();
@@ -495,23 +484,7 @@ __global__ void __launch_bounds__(128) alz_lpc_levinson_kernel(const __grid_cons
 // After a call's frames: per stream (one CTA), the last `size` samples and the sample count.
 __global__ void __launch_bounds__(kThreadsCommit) alz_lpc_commit_kernel(const __grid_constant__ LpcArgs a) {
   extern __shared__ float s_t[];
-  const long long s = blockIdx.x;
-  unsigned char* st = a.state + s * a.sstride;
-  const long long C = *reinterpret_cast<const long long*>(st), C1 = C + a.T;
-  float* tail = reinterpret_cast<float*>(st + 16);
-  const float* xr = a.x + s * a.xs;
-  for (int j = threadIdx.x; j < a.size; j += blockDim.x) {
-    const long long g = C1 - a.size + j;
-    s_t[j] = g >= C ? xr[g - C] : (g >= C - a.size ? tail[g - (C - a.size)] : 0.f);
-  }
-  __syncthreads();
-  for (int j = threadIdx.x; j < a.size; j += blockDim.x) tail[j] = s_t[j];
-  if (threadIdx.x == 0) *reinterpret_cast<long long*>(st) = C1;
-}
-
-__global__ void __launch_bounds__(kThreadsCommit) alz_lpc_init_kernel(unsigned char* state, long long n_words) {
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n_words; i += (long long)gridDim.x * blockDim.x)
-    reinterpret_cast<int*>(state)[i] = 0;
+  framed_commit(a.state + blockIdx.x * a.sstride, a.x + blockIdx.x * a.xs, a.T, a.size, s_t);
 }
 
 extern "C" {
@@ -527,7 +500,7 @@ int64_t alz_lpc_frames(int64_t consumed, int64_t n_samples, int32_t size, int32_
 int64_t alz_lpc_state_bytes(int64_t n_streams, int32_t size) {
   if (n_streams < 0 || size < 1 || size > ALZ_LPC_MAX_SIZE)
     return fail(ALZ_LPC_ERR_INVALID, "need n_streams >= 0 and 1 <= size <= %d", ALZ_LPC_MAX_SIZE);
-  return n_streams * state_stride(size);
+  return n_streams * framed_state_stride(size);
 }
 
 int32_t alz_lpc_state_init(void* state_dev, int64_t n_streams, int32_t size, void* cuda_stream) {
@@ -535,10 +508,8 @@ int32_t alz_lpc_state_init(void* state_dev, int64_t n_streams, int32_t size, voi
     return fail(ALZ_LPC_ERR_INVALID, "need n_streams >= 0 and 1 <= size <= %d", ALZ_LPC_MAX_SIZE);
   if (n_streams == 0) return ALZ_LPC_OK;
   if (!state_dev || ((uintptr_t)state_dev & 7)) return fail(ALZ_LPC_ERR_INVALID, "state is NULL or not 8-byte aligned");
-  const long long n = n_streams * (state_stride(size) / 4);
-  const unsigned blocks = (unsigned)((n + kThreadsCommit - 1) / kThreadsCommit < 4096 ? (n + kThreadsCommit - 1) / kThreadsCommit : 4096);
-  alz_lpc_init_kernel<<<blocks, kThreadsCommit, 0, (cudaStream_t)cuda_stream>>>((unsigned char*)state_dev, n);
-  ALZ_CUDA_CHECK(cudaGetLastError(), ALZ_LPC_ERR_CUDA);
+  ALZ_CUDA_CHECK(cudaMemsetAsync(state_dev, 0, n_streams * framed_state_stride(size), (cudaStream_t)cuda_stream),
+                 ALZ_LPC_ERR_CUDA);
   return ALZ_LPC_OK;
 }
 
@@ -599,7 +570,7 @@ int32_t run(bool covar, const float* x_dev, int64_t x_stride, const double* wind
   a.failed = failed_dev;
   a.state = (unsigned char*)state_dev;
   a.xs = x_stride;
-  a.sstride = state_stride(size);
+  a.sstride = framed_state_stride(size);
   a.T = n_samples;
   a.F = n_frames;
   a.order = order;
@@ -617,9 +588,7 @@ int32_t run(bool covar, const float* x_dev, int64_t x_stride, const double* wind
     int threads = (a.fpc * a.ncell + 31) / 32 * 32;
     if (threads > kMaxFramesPerCta * 32) threads = kMaxFramesPerCta * 32;
     const size_t smem = (size_t)a.fpc * (size + 1) * 8;
-    if (smem > 48 * 1024)
-      ALZ_CUDA_CHECK(cudaFuncSetAttribute(alz_lpc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
-                     ALZ_LPC_ERR_CUDA);
+    ALZ_CUDA_CHECK(allow_dynamic_smem((const void*)alz_lpc_kernel, smem), ALZ_LPC_ERR_CUDA);
     alz_lpc_kernel<<<(unsigned)grid, threads, smem, cs>>>(a);
     ALZ_CUDA_CHECK(cudaGetLastError(), ALZ_LPC_ERR_CUDA);
     if (solve) {
@@ -638,9 +607,7 @@ int32_t run(bool covar, const float* x_dev, int64_t x_stride, const double* wind
         blocks = (total + nt - 1) / nt;
       }
       if (blocks > 0x7fffffffLL) return fail(ALZ_LPC_ERR_UNSUPPORTED, "too many frames for one launch");
-      if (smem2 > 48 * 1024)
-        ALZ_CUDA_CHECK(cudaFuncSetAttribute(alz_lpc_levinson_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                            (int)smem2), ALZ_LPC_ERR_CUDA);
+      ALZ_CUDA_CHECK(allow_dynamic_smem((const void*)alz_lpc_levinson_kernel, smem2), ALZ_LPC_ERR_CUDA);
       alz_lpc_levinson_kernel<<<(unsigned)blocks, nt, smem2, cs>>>(a, total);
       ALZ_CUDA_CHECK(cudaGetLastError(), ALZ_LPC_ERR_CUDA);
     }

@@ -23,15 +23,12 @@
 #include <algorithm>
 #include <cmath>
 #include <cstdint>
-#include <mutex>
-#include <set>
 
 namespace {
 
 constexpr int kTile = 128;                  // outputs per CTA (one per thread)
 constexpr int kGroup = 8;                   // streams per CTA: the tile's weights are staged once for all of them
 constexpr int kThreadsCommit = 64;
-constexpr int kMaxSmem = (ALZ_RESAMPLE_MAX_ORDER + 1) * kTile * (int)sizeof(double);
 
 struct ResampleArgs {
   const float* x;
@@ -107,45 +104,15 @@ __global__ void __launch_bounds__(kTile) alz_resample_kernel(const __grid_consta
   }
 }
 
-// The history becomes the last L samples of (history, block).  In place, ascending: new[i] reads old[i + T], which no
-// earlier pass has written.
+// The history becomes the last L samples of (history, block).
 __global__ void __launch_bounds__(kThreadsCommit) alz_resample_commit_kernel(const __grid_constant__ ResampleArgs a) {
-  double* hist = a.state + (long long)blockIdx.x * a.L;
-  const float* xr = a.x + (long long)blockIdx.x * a.xs;
-  for (int i0 = 0; i0 < a.L; i0 += kThreadsCommit) {
-    const int i = i0 + threadIdx.x;
-    const long long p = a.T - a.L + i;
-    double v = 0.0;
-    if (i < a.L) v = p >= 0 ? (double)xr[p] : hist[i + a.T];
-    __syncthreads();
-    if (i < a.L) hist[i] = v;
-    __syncthreads();
-  }
+  shift_history(a.state + (long long)blockIdx.x * a.L, a.L, a.x + (long long)blockIdx.x * a.xs, a.T);
 }
 
 __global__ void __launch_bounds__(256) alz_resample_init_kernel(double* state, long long n, double zero) {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
     state[i] = zero;
 }
-
-namespace {
-
-// The interpolation kernel's dynamic shared-memory limit is raised once per device to what order 64 needs (66.5 KB,
-// above the 48 KB default); each launch asks for its own order's size.
-cudaError_t allow_max_smem() {
-  static std::mutex mu;
-  static std::set<int> done;
-  int dev = -1;
-  cudaError_t e = cudaGetDevice(&dev);
-  if (e != cudaSuccess) return e;
-  std::lock_guard<std::mutex> lock(mu);
-  if (done.count(dev)) return cudaSuccess;
-  e = cudaFuncSetAttribute(alz_resample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
-  if (e == cudaSuccess) done.insert(dev);
-  return e;
-}
-
-}  // namespace
 
 extern "C" {
 
@@ -230,11 +197,11 @@ int32_t alz_resample_apply(const float* x_dev, void* out_dev, int32_t out_f64, d
   if (tiles > 0x7fffffffLL || n_streams > 0x7fffffffLL) return fail(ALZ_RESAMPLE_ERR_UNSUPPORTED, "too large a block for one launch");
   const cudaStream_t st = (cudaStream_t)cuda_stream;
   if (n_out > 0) {
-    ALZ_CUDA_CHECK(allow_max_smem(), ALZ_RESAMPLE_ERR_CUDA);
     const unsigned wblocks = (unsigned)std::min<long long>((n_out + 255) / 256, 8192);
     alz_resample_weights_kernel<<<wblocks, 256, 0, st>>>(idx_dev, weights_dev, n_out, a.L);
     ALZ_CUDA_CHECK(cudaGetLastError(), ALZ_RESAMPLE_ERR_CUDA);
     const size_t smem = (size_t)a.L * kTile * sizeof(double);
+    ALZ_CUDA_CHECK(allow_dynamic_smem((const void*)alz_resample_kernel, smem), ALZ_RESAMPLE_ERR_CUDA);
     alz_resample_kernel<<<dim3((unsigned)tiles, (unsigned)groups), kTile, smem, st>>>(a);
     ALZ_CUDA_CHECK(cudaGetLastError(), ALZ_RESAMPLE_ERR_CUDA);
   }

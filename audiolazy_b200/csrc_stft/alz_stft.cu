@@ -12,8 +12,8 @@
 //   * alz_ola_kernel: one thread per output sample of a stream sums the frames that cover it, oldest first, starting
 //     from the open sum the state holds for the first size - hop samples; the sums still open after the call are
 //     written to the state's other copy;
-//   * alz_ola_commit_kernel: per stream, flips the state's copy and counts the frames;
-//   * alz_stft_init_kernel: zeroes a state.
+//   * alz_ola_commit_kernel: per stream, flips the state's copy and counts the frames.
+// Both states start as zero bytes (cudaMemsetAsync).
 //
 // The transform is a mixed-radix decimation in time, in place in one shared buffer of N complex values (size 8192
 // takes 128 KB): radices 4, 2, 3, 5, 7, then the other primes.  The frame is loaded in digit-reversed order
@@ -72,7 +72,6 @@ struct OlaArgs {
   int size, hop, final_;
 };
 
-long long state_stride(int size) { return (16 + 4 * (long long)size + 7) / 8 * 8; }
 long long ola_state_stride(int size, int hop) { return 16 + 16 * (long long)(size - hop); }
 
 Fft factor(int n) {
@@ -255,11 +254,8 @@ __global__ void __launch_bounds__(kMaxThreads) alz_stft_analysis_kernel(const __
   extern __shared__ double2 s_buf[];           // [fpc][size]
   const long long s = blockIdx.x / a.blocks_per_stream;
   const long long i0 = (long long)(blockIdx.x % a.blocks_per_stream) * a.fpc;
-  const unsigned char* st = a.state + s * a.sstride;
-  const long long C = *reinterpret_cast<const long long*>(st);
-  const float* tail = reinterpret_cast<const float*>(st + 16);    // samples [C - size, C)
-  const float* xr = a.x + s * a.xs;
-  const long long ka = first_open_block(C, a.size, a.hop);
+  const FramedSamples in = framed_samples(a.state + s * a.sstride, a.x + s * a.xs, a.T, a.size);
+  const long long ka = first_open_block(in.C, a.size, a.hop);
   const int N = a.size, half = N / 2;
   const int nf = (int)(a.F - i0 < a.fpc ? a.F - i0 : a.fpc);
   const int f = threadIdx.x / a.tpf, tid = threadIdx.x - f * a.tpf;
@@ -269,13 +265,7 @@ __global__ void __launch_bounds__(kMaxThreads) alz_stft_analysis_kernel(const __
   if (active) {
     const long long g0 = (ka + i0 + f) * a.hop;                     // stream index of the frame's sample 0
     for (int n = tid; n < N; n += a.tpf) {
-      const long long g = g0 + n;
-      float v = 0.f;
-      if (g < C) {
-        v = tail[g - (C - N)];
-      } else if (g < C + a.T) {
-        v = xr[g - C];
-      }
+      const float v = in(g0 + n);
       const double b = a.w ? __dmul_rn((double)v, a.w[n]) : (double)v;
       int p = n;
       if (a.shift) p = n >= half ? n - half : n + (N - half);     // b'[p] = b[(p + half) % N]
@@ -379,23 +369,7 @@ __global__ void alz_ola_commit_kernel(unsigned char* state, long long sstride, l
 // After an analysis call: per stream (one CTA), the last `size` samples and the sample count.
 __global__ void __launch_bounds__(kThreadsCommit) alz_stft_commit_kernel(const __grid_constant__ StftArgs a) {
   extern __shared__ float s_t[];
-  const long long s = blockIdx.x;
-  unsigned char* st = a.state + s * a.sstride;
-  const long long C = *reinterpret_cast<const long long*>(st), C1 = C + a.T;
-  float* tail = reinterpret_cast<float*>(st + 16);
-  const float* xr = a.x + s * a.xs;
-  for (int j = threadIdx.x; j < a.size; j += blockDim.x) {
-    const long long g = C1 - a.size + j;
-    s_t[j] = g >= C ? xr[g - C] : (g >= C - a.size ? tail[g - (C - a.size)] : 0.f);
-  }
-  __syncthreads();
-  for (int j = threadIdx.x; j < a.size; j += blockDim.x) tail[j] = s_t[j];
-  if (threadIdx.x == 0) *reinterpret_cast<long long*>(st) = C1;
-}
-
-__global__ void __launch_bounds__(kThreadsCommit) alz_stft_init_kernel(unsigned char* state, long long n_words) {
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n_words; i += (long long)gridDim.x * blockDim.x)
-    reinterpret_cast<int*>(state)[i] = 0;
+  framed_commit(a.state + blockIdx.x * a.sstride, a.x + blockIdx.x * a.xs, a.T, a.size, s_t);
 }
 
 namespace {
@@ -407,12 +381,10 @@ int check_shape(int32_t size, int32_t hop) {
   return ALZ_STFT_OK;
 }
 
-int32_t init_state(void* state_dev, long long n_words, cudaStream_t cs) {
-  if (n_words == 0) return ALZ_STFT_OK;
+int32_t init_state(void* state_dev, long long bytes, cudaStream_t cs) {
+  if (bytes == 0) return ALZ_STFT_OK;
   if (!state_dev || ((uintptr_t)state_dev & 7)) return fail(ALZ_STFT_ERR_INVALID, "state is NULL or not 8-byte aligned");
-  const long long b = (n_words + kThreadsCommit - 1) / kThreadsCommit;
-  alz_stft_init_kernel<<<(unsigned)(b < 4096 ? b : 4096), kThreadsCommit, 0, cs>>>((unsigned char*)state_dev, n_words);
-  ALZ_CUDA_CHECK(cudaGetLastError(), ALZ_STFT_ERR_CUDA);
+  ALZ_CUDA_CHECK(cudaMemsetAsync(state_dev, 0, bytes, cs), ALZ_STFT_ERR_CUDA);
   return ALZ_STFT_OK;
 }
 
@@ -425,9 +397,7 @@ int32_t launch_frames(const void* kernel, StftArgs& a, long long n_streams, cuda
   const long long grid = n_streams * a.blocks_per_stream;
   if (grid > 0x7fffffffLL || a.F > 0x7fffffffLL) return fail(ALZ_STFT_ERR_UNSUPPORTED, "too many frames for one launch");
   const size_t smem = (size_t)a.fpc * a.size * 16;
-  if (smem > 48 * 1024)
-    ALZ_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
-                   ALZ_STFT_ERR_CUDA);
+  ALZ_CUDA_CHECK(allow_dynamic_smem(kernel, smem), ALZ_STFT_ERR_CUDA);
   void* args[] = {&a};
   ALZ_CUDA_CHECK(cudaLaunchKernel(kernel, dim3((unsigned)grid), dim3(a.fpc * a.tpf), args, smem, cs), ALZ_STFT_ERR_CUDA);
   return ALZ_STFT_OK;
@@ -487,13 +457,13 @@ int64_t alz_stft_frames(int64_t consumed, int64_t n_samples, int32_t size, int32
 int64_t alz_stft_analysis_state_bytes(int64_t n_streams, int32_t size) {
   if (n_streams < 0 || size < 1 || size > ALZ_STFT_MAX_SIZE)
     return fail(ALZ_STFT_ERR_INVALID, "need n_streams >= 0 and 1 <= size <= %d", ALZ_STFT_MAX_SIZE);
-  return n_streams * state_stride(size);
+  return n_streams * framed_state_stride(size);
 }
 
 int32_t alz_stft_analysis_state_init(void* state_dev, int64_t n_streams, int32_t size, void* cuda_stream) {
   const int64_t n = alz_stft_analysis_state_bytes(n_streams, size);
   if (n < 0) return (int32_t)n;
-  return init_state(state_dev, n / 4, (cudaStream_t)cuda_stream);
+  return init_state(state_dev, n, (cudaStream_t)cuda_stream);
 }
 
 int64_t alz_stft_ola_state_bytes(int64_t n_streams, int32_t size, int32_t hop) {
@@ -505,7 +475,7 @@ int64_t alz_stft_ola_state_bytes(int64_t n_streams, int32_t size, int32_t hop) {
 int32_t alz_stft_ola_state_init(void* state_dev, int64_t n_streams, int32_t size, int32_t hop, void* cuda_stream) {
   const int64_t n = alz_stft_ola_state_bytes(n_streams, size, hop);
   if (n < 0) return (int32_t)n;
-  return init_state(state_dev, n / 4, (cudaStream_t)cuda_stream);
+  return init_state(state_dev, n, (cudaStream_t)cuda_stream);
 }
 
 int32_t alz_stft_analysis(const float* x_dev, int64_t x_stride, const double* window_dev, const double* twiddle_dev,
@@ -528,7 +498,7 @@ int32_t alz_stft_analysis(const float* x_dev, int64_t x_stride, const double* wi
   a.spec_out = spec_dev;
   a.state = (unsigned char*)state_dev;
   a.xs = x_stride;
-  a.sstride = state_stride(size);
+  a.sstride = framed_state_stride(size);
   a.T = n_samples;
   a.F = n_frames;
   a.size = size;

@@ -252,7 +252,7 @@ MAX_ORDER = 64
 MAX_SIZE = 8192
 
 _i32, _i64, _vp = ctypes.c_int32, ctypes.c_int64, ctypes.c_void_p
-LIB = _capi.NativeLib(_build.LPC_LIB_PATH, "LPC", {
+LIB = _capi.NativeLib(_build.LIBRARIES["lpc"].path, "LPC", {
   "alz_lpc_last_error": (ctypes.c_char_p, []),
   "alz_lpc_frames": (_i64, [_i64, _i64, _i32, _i32, _i32]),
   "alz_lpc_state_bytes": (_i64, [_i64, _i32]),

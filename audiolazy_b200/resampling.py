@@ -37,7 +37,7 @@ ERR_UNSUPPORTED = _capi.ALZ_ERR_UNSUPPORTED
 ERR_CAPACITY = -7
 
 _i32, _i64, _f64, _vp = ctypes.c_int32, ctypes.c_int64, ctypes.c_double, ctypes.c_void_p
-LIB = _capi.NativeLib(_build.RESAMPLE_LIB_PATH, "resampling", {
+LIB = _capi.NativeLib(_build.LIBRARIES["resample"].path, "resampling", {
   "alz_resample_last_error": (ctypes.c_char_p, []),
   "alz_resample_state_doubles": (_i64, [_i32, _i64]),
   "alz_resample_state_init": (_i32, [_vp, _i64, _i32, _f64, _vp]),

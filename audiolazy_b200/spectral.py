@@ -161,7 +161,7 @@ def ola_window(size, hop, wnd=None, normalize=True, strategy="numpy"):
 MAX_SIZE = 8192
 
 _i32, _i64, _vp = ctypes.c_int32, ctypes.c_int64, ctypes.c_void_p
-LIB = _capi.NativeLib(_build.STFT_LIB_PATH, "STFT", {
+LIB = _capi.NativeLib(_build.LIBRARIES["stft"].path, "STFT", {
   "alz_stft_last_error": (ctypes.c_char_p, []),
   "alz_stft_frames": (_i64, [_i64, _i64, _i32, _i32, _i32]),
   "alz_stft_analysis_state_bytes": (_i64, [_i64, _i32]),

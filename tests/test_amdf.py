@@ -10,10 +10,9 @@ import numpy as np
 import pytest
 
 import audiolazy_b200 as ab
-from audiolazy_b200 import _build, analysis as amdf_mod
+from audiolazy_b200 import analysis as amdf_mod
 from amdf_emulation import amdf as emulate, digest
 from conftest import GOLDEN
-from native_libs import check_exports, check_sm90a
 
 
 @pytest.fixture(scope="module")
@@ -81,11 +80,3 @@ def test_freq2lag_lag2freq():
   s, Hz = ab.sHz(48000)
   assert abs(ab.freq2lag(1000 * Hz) - 48.0) < 1e-12
   assert ab.freq2lag(2 * math.pi / 37.25) == 2 * math.pi / (2 * math.pi / 37.25)
-
-
-def test_amdf_library_exports_exactly_its_header():
-  check_exports(amdf_mod.LIB, "alz_b200_amdf.h")
-
-
-def test_amdf_library_is_sm90a():
-  check_sm90a(_build.AMDF_LIB_PATH)

@@ -778,3 +778,58 @@ def test_plans_dropped_while_their_launches_are_queued(world, churn, torch):
   _same(out["window"], want_w, "window plan dropped")
   _same(out["generic"], want_g, "generic plan dropped")
   _same({"out": out["amdf"]}, {"out": want_amdf}, "AmdfBank dropped")
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# (h) launches above the 48 KB shared-memory default, of different sizes, from two threads
+# ---------------------------------------------------------------------------------------------------------------------
+def _frames_job(lp, x):
+  def run():
+    st = lp.new_state(x.shape[0])
+    res = lp.apply(x, state=st, final=True)
+    return {"coef": res[0], "error": res[1], "failed": res[2], "state": st.tensor}
+  return run
+
+
+def _stft_job(stft, x):
+  def run():
+    st = stft.new_state(x.shape[0])
+    spec = stft.analyze(x, st, final=True)
+    y = stft.synthesize(spec, st, final=True)
+    return {"spec": spec, "y": y, "state": st.tensor, "ola_state": st.ola.tensor}
+  return run
+
+
+def test_two_threads_launch_one_kernel_with_different_sizes_above_48_kb(torch):
+  """Thread A runs LPC frames of 8192 samples (64 KiB of dynamic shared memory for a frame) and an STFT of size 8192
+  (128 KiB); thread B LPC frames of 7000 samples (about 55 KiB), an STFT of size 4096 (64 KiB) and kcovar at order 64
+  (68 KiB a warp in the recursion).  Each job makes launches above the 48 KB default, and the two threads launch the
+  same kernels with different sizes at once: each launch must find the kernel's limit at least as high as its own
+  size, whatever the other thread launched last.  Three calls of each job per thread, each result equal to the serial
+  one."""
+  rng = np.random.default_rng(31)
+
+  def dev(*shape):
+    return torch.from_numpy(rng.uniform(-1, 1, shape).astype(np.float32)).cuda()
+  jobs = [
+    {"lpc-8192": _frames_job(ab.LpcFrames(16, 8192, 4096, np.hanning(8192)), dev(4, 3 * 8192)),
+     "stft-8192": _stft_job(ab.Stft(8192, 2048, wnd=ab.window.hann, dtype=torch.complex128), dev(4, 3 * 8192))},
+    {"lpc-7000": _frames_job(ab.LpcFrames(12, 7000, 3000), dev(4, 3 * 7000)),
+     "stft-4096": _stft_job(ab.Stft(4096, 1024, wnd=ab.window.hann, dtype=torch.complex128), dev(4, 3 * 4096)),
+     "kcovar-64": _frames_job(ab.LpcFrames(64, 512, 256, method="kcovar"), dev(4, 8192))}]
+  serial = {}
+  for mine in jobs:
+    for name, run in mine.items():
+      serial[name] = run()
+  torch.cuda.synchronize()
+  streams = [torch.cuda.Stream(), torch.cuda.Stream(priority=-1)]
+
+  def worker(i):
+    def body():
+      for r in range(ROUNDS):
+        for name, run in jobs[i].items():
+          got = _on(streams[i], run)
+          streams[i].synchronize()
+          _same(got, serial[name], "thread %d, round %d, %s" % (i, r, name))
+    return body
+  _run_threads([worker(0), worker(1)])

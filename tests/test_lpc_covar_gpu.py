@@ -240,4 +240,4 @@ for name in sorted({e.name.split("(")[0].strip() for e in prof.events() if e.nam
 
 
 def test_both_methods_launch_exactly_the_library_kernels(torch):
-  check_every_kernel_is_launched(_build.LPC_LIB_PATH, _LAUNCH_PROBE)
+  check_every_kernel_is_launched(_build.LIBRARIES["lpc"].path, _LAUNCH_PROBE)

@@ -14,7 +14,7 @@ import pytest
 import audiolazy_b200 as ab
 from audiolazy_b200 import _build, crossing, linear_prediction as lp
 from conftest import GOLDEN
-from native_libs import check_exports, check_sm90a, cuobjdump
+from native_libs import cuobjdump
 import lpc_emulation as em
 
 sys.path.insert(0, GOLDEN)
@@ -117,20 +117,12 @@ def test_library_sizes_without_a_device():
   assert "order" in L.alz_lpc_last_error().decode()
 
 
-def test_lpc_library_exports_exactly_its_header():
-  check_exports(lp.LIB, "alz_b200_lpc.h")
-
-
-def test_lpc_library_is_sm90a():
-  check_sm90a(_build.LPC_LIB_PATH)
-
-
 def test_lpc_library_has_no_fused_multiply_add():
   """Built with -fmad=false: no product is contracted into an add, as the reference's arithmetic requires.  The only
   DFMAs are the Newton steps of the one correctly rounded division in the Levinson-Durbin kernel (c = num / den)."""
-  sass = subprocess.run([cuobjdump(), "-sass", _build.LPC_LIB_PATH], capture_output=True, text=True).stdout
+  sass = subprocess.run([cuobjdump(), "-sass", _build.LIBRARIES["lpc"].path], capture_output=True, text=True).stdout
   functions = re.split(r"\n\s*Function : ", sass)[1:]
-  assert len(functions) == 4
+  assert len(functions) == 3
   by_name = {f.split(None, 1)[0]: f for f in functions}
   lev = [body for name, body in by_name.items() if "alz_lpc_levinson_kernel" in name]
   acorr = [body for name, body in by_name.items() if "alz_lpc_kernel" in name]

@@ -219,4 +219,4 @@ for name in sorted({e.name.split("(")[0].strip() for e in prof.events() if e.nam
 
 
 def test_every_lpc_kernel_is_launched(torch):
-  check_every_kernel_is_launched(_build.LPC_LIB_PATH, _LAUNCH_PROBE)
+  check_every_kernel_is_launched(_build.LIBRARIES["lpc"].path, _LAUNCH_PROBE)

@@ -1,20 +1,33 @@
-"""Every native library of ``_build.LIBRARIES``: it has a Python binding, that binding fails loudly when the library
-cannot be loaded (there is no CPU fallback), and the library is rebuilt when a source it depends on changes.  Each
-library's exports, target and kernel launches are checked next to its other tests (``native_libs.check_*``)."""
+"""Every native library of ``_build.LIBRARIES``: it has a Python binding that binds exactly the functions its header
+declares, the library exports them and targets sm_90a, the binding fails loudly when the library cannot be loaded
+(there is no CPU fallback), and the library is rebuilt when a source it depends on changes.  Each library's kernel
+launches are checked next to its GPU tests (``native_libs.check_every_kernel_is_launched``)."""
 import os
 import shutil
 
 import pytest
 
-from audiolazy_b200 import _build, _capi, analysis, crossing, linear_prediction
+from audiolazy_b200 import _build, _capi, analysis, crossing, linear_prediction, resampling, spectral
 from conftest import ROOT
+from native_libs import check_exports, check_sm90a
 
 NAMES = sorted(_build.LIBRARIES)
-BINDINGS = {"filters": _capi.LIB, "amdf": analysis.LIB, "zcross": crossing.LIB, "lpc": linear_prediction.LIB}
+BINDINGS = {"filters": _capi.LIB, "amdf": analysis.LIB, "zcross": crossing.LIB, "lpc": linear_prediction.LIB,
+            "stft": spectral.LIB, "resample": resampling.LIB}
 
 
 def test_every_library_has_a_binding():
   assert sorted(BINDINGS) == NAMES
+
+
+@pytest.mark.parametrize("name", NAMES)
+def test_library_exports_exactly_its_header(name):
+  check_exports(BINDINGS[name], _build.LIBRARIES[name].header)
+
+
+@pytest.mark.parametrize("name", NAMES)
+def test_library_is_sm90a(name):
+  check_sm90a(_build.LIBRARIES[name].path)
 
 
 @pytest.mark.parametrize("name", NAMES)
@@ -34,7 +47,7 @@ def test_unloadable_library_raises_native_error(name, tmp_path, monkeypatch):
 
 
 def test_staleness_follows_the_dependencies(tmp_path, monkeypatch):
-  """In a copy of the sources: touching the shared header marks exactly the three analysis libraries stale, touching
+  """In a copy of the sources: touching the shared header marks exactly the five analysis libraries stale, touching
   one library's unit or public header marks only that library stale."""
   for d in ("include", "audiolazy_b200"):
     shutil.copytree(os.path.join(ROOT, d), str(tmp_path / d), ignore=shutil.ignore_patterns("_native", "__pycache__"))
@@ -53,7 +66,10 @@ def test_staleness_follows_the_dependencies(tmp_path, monkeypatch):
     os.utime(str(tmp_path / rel), (3000, 3000))
     return sorted(lib.name for lib in libs if _build.is_stale(lib))
 
-  assert stale_after_touching("audiolazy_b200/csrc_common/alz_common.h") == ["amdf", "lpc", "zcross"]
+  assert stale_after_touching("audiolazy_b200/csrc_common/alz_common.h") == ["amdf", "lpc", "resample", "stft", "zcross"]
   assert stale_after_touching("audiolazy_b200/csrc_lpc/alz_lpc.cu") == ["lpc"]
   assert stale_after_touching("include/alz_b200_zcross.h") == ["zcross"]
   assert stale_after_touching("audiolazy_b200/csrc/alz_plan.h") == ["filters"]
+  assert stale_after_touching("audiolazy_b200/csrc_stft/alz_stft.cu") == ["stft"]
+  assert stale_after_touching("include/alz_b200_stft.h") == ["stft"]
+  assert stale_after_touching("audiolazy_b200/csrc_resample/alz_resample.cu") == ["resample"]

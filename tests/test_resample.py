@@ -1,7 +1,6 @@
 """resample / lagrange against the reference's goldens on the CPU: the float64 emulation of the header's arithmetic
 reproduces every digest (in one block and cut into blocks), lagrange's values and polynomial coefficients equal the
-reference's, the library's host schedule equals the emulation's bit for bit, the reference's errors and the checks
-every native library takes, applied to libalz_b200_resample.so."""
+reference's, the library's host schedule equals the emulation's bit for bit, and the reference's errors."""
 import builtins
 import json
 import math
@@ -13,11 +12,10 @@ import numpy as np
 import pytest
 
 import audiolazy_b200 as ab
-from audiolazy_b200 import _build, _capi, resampling
+from audiolazy_b200 import resampling
 from conftest import GOLDEN
 import resample_emulation as em
 from lpc_emulation import digest
-from native_libs import check_exports, check_sm90a
 
 sys.path.insert(0, GOLDEN)
 import make_resample  # noqa: E402
@@ -127,22 +125,6 @@ def test_unsupported_steps_raise_not_implemented():
     ab.Resampler(1, 2, order=65)
   with pytest.raises(ValueError):
     ab.Resampler(1, 2, order=0)
-
-
-def test_resample_exports():
-  check_exports(resampling.LIB, "alz_b200_resample.h")
-
-
-def test_resample_targets_sm90a():
-  check_sm90a(_build.RESAMPLE_LIB_PATH)
-
-
-def test_unloadable_resample_library_raises_native_error(tmp_path, monkeypatch):
-  binding = resampling.LIB
-  monkeypatch.setattr(binding, "cdll", None)
-  monkeypatch.setattr(binding, "path", str(tmp_path / "missing.so"))
-  with pytest.raises(_capi.NativeError, match="no CPU fallback"):
-    binding.load()
 
 
 def test_vectorised_emulation_reproduces_every_digest(golden, inputs):

@@ -1,19 +1,16 @@
 """window / wsymm and the overlap-add gains against the reference's goldens, the numpy emulation of overlap_add against
-the reference's outputs, the frame-count rule, the reference's errors, and the checks every native library takes,
-applied to libalz_b200_stft.so (which sits next to ``_build.LIBRARIES``, not in it)."""
+the reference's outputs, the frame-count rule and the reference's errors."""
 import json
 import math
 import os
-import shutil
 
 import numpy as np
 import pytest
 
 import audiolazy_b200 as ab
-from audiolazy_b200 import _build, _capi, _engine, spectral
-from conftest import GOLDEN, ROOT
+from audiolazy_b200 import _engine, spectral
+from conftest import GOLDEN
 import stft_emulation as em
-from native_libs import check_exports, check_sm90a
 
 
 @pytest.fixture(scope="module")
@@ -138,48 +135,3 @@ def test_reference_errors_at_call_time():
       ab.stft[name](abs, size=4)
   assert ab.stft.base is ab.stft.real is ab.stft.rfft is ab.stft.default
 
-
-def test_stft_exports():
-  check_exports(spectral.LIB, "alz_b200_stft.h")
-
-
-def test_stft_targets_sm90a():
-  check_sm90a(_build.STFT_LIB_PATH)
-
-
-def test_unloadable_stft_library_raises_native_error(tmp_path, monkeypatch):
-  binding = spectral.LIB
-  monkeypatch.setattr(binding, "cdll", None)
-  monkeypatch.setattr(binding, "path", str(tmp_path / "missing.so"))
-  with pytest.raises(_capi.NativeError, match="no CPU fallback"):
-    binding.load()
-  junk = tmp_path / "junk.so"
-  junk.write_text("not an ELF file\n")
-  monkeypatch.setattr(binding, "path", str(junk))
-  with pytest.raises(_capi.NativeError, match="cannot load"):
-    binding.load()
-
-
-def test_staleness_of_the_stft_library(tmp_path, monkeypatch):
-  """Touching the STFT unit or header marks only it stale among the five libraries; touching the shared header marks
-  it and the three analysis libraries."""
-  for d in ("include", "audiolazy_b200"):
-    shutil.copytree(os.path.join(ROOT, d), str(tmp_path / d), ignore=shutil.ignore_patterns("_native", "__pycache__"))
-  monkeypatch.setattr(_build, "ROOT", str(tmp_path))
-  libs = list(_build.LIBRARIES.values()) + [_build.STFT]
-  os.makedirs(str(tmp_path / _build.NATIVE))
-  for lib in libs:
-    open(lib.path, "w").close()
-
-  def stale_after_touching(rel):
-    for lib in libs:
-      for src in lib.units() + lib.headers():
-        os.utime(src, (1000, 1000))
-      os.utime(lib.path, (2000, 2000))
-    assert not any(_build.is_stale(lib) for lib in libs)
-    os.utime(str(tmp_path / rel), (3000, 3000))
-    return sorted(lib.name for lib in libs if _build.is_stale(lib))
-
-  assert stale_after_touching("audiolazy_b200/csrc_stft/alz_stft.cu") == ["stft"]
-  assert stale_after_touching("include/alz_b200_stft.h") == ["stft"]
-  assert stale_after_touching("audiolazy_b200/csrc_common/alz_common.h") == ["amdf", "lpc", "stft", "zcross"]

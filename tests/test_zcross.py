@@ -10,9 +10,8 @@ import numpy as np
 import pytest
 
 import audiolazy_b200 as ab
-from audiolazy_b200 import _build, crossing
+from audiolazy_b200 import crossing
 from conftest import GOLDEN
-from native_libs import check_exports, check_sm90a
 from zcross_emulation import block_sums, digest, zcross as emulate
 
 sys.path.insert(0, GOLDEN)
@@ -93,14 +92,6 @@ def test_n_blocks_matches_the_emulated_split(consumed, T, size, hop, final):
   before = len(block_sums(flags[:consumed], size, hop, final=False))
   total = len(block_sums(flags, size, hop, final=final))
   assert crossing.n_blocks(consumed, T, size, hop, final) == total - before
-
-
-def test_zcross_library_exports_exactly_its_header():
-  check_exports(crossing.LIB, "alz_b200_zcross.h")
-
-
-def test_zcross_library_is_sm90a():
-  check_sm90a(_build.ZCROSS_LIB_PATH)
 
 
 def test_library_sizes_without_a_device():
