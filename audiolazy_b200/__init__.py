@@ -10,10 +10,11 @@ batched form ``Zcross`` (flags or per-block counts of many streams); ``lpc_frame
 (``lpc.kautocor`` or ``lpc.kcovar`` of every block of many streams); ``window`` / ``wsymm``, ``overlap_add`` and
 ``stft`` with their batched forms ``OverlapAdd`` and ``Stft`` (short-time Fourier analysis, resynthesis and
 overlap-add of many streams); ``lagrange`` and ``resample`` with its batched form ``Resampler`` (Lagrange sample-rate
-conversion of many streams).
+conversion of many streams); ``dft`` at arbitrary frequencies with its batched form ``Dft`` and the lazy ``dft_frames``
+(the DFT of every frame of many streams).
 
 The per-sample recurrences run in hand-written sm_90a CUDA kernels behind the C ABIs of
-``include/alz_b200.h``, ``include/alz_b200_amdf.h``, ``include/alz_b200_zcross.h``, ``include/alz_b200_lpc.h``, ``include/alz_b200_stft.h`` and ``include/alz_b200_resample.h``; importing this package does not need a GPU, calling a filter does.
+``include/alz_b200.h``, ``include/alz_b200_amdf.h``, ``include/alz_b200_zcross.h``, ``include/alz_b200_lpc.h``, ``include/alz_b200_stft.h``, ``include/alz_b200_resample.h`` and ``include/alz_b200_dft.h``; importing this package does not need a GPU, calling a filter does.
 """
 from .core import StrategyDict
 from .stream import Stream, StreamTeeHub, thub, tostream, avoid_stream
@@ -31,5 +32,6 @@ from .linear_prediction import (ParCorError, acorr, lag_matrix, toeplitz, levins
                                 lsf, lsf_stable, LpcFrames, LpcState, lpc_frames)
 from .spectral import window, wsymm, overlap_add, stft, OverlapAdd, OlaState, Stft, StftState
 from .resampling import lagrange, resample, Resampler, ResampleState
+from .fourier import dft, Dft, DftState, dft_frames
 
 __version__ = "0.1.0"

@@ -20,6 +20,11 @@ parallel into ``_native/obj/<name>/`` (only the units that changed) and linked i
   AudioLazy's bit for bit).
 
 The five analysis libraries also include ``csrc_common/alz_common.h``.
+
+:data:`DFT` is a seventh library, declared next to the table rather than in it: ``libalz_b200_dft.so``, the DFT
+library: ``csrc_dft/*.cu`` behind ``include/alz_b200_dft.h``, compiled with ``-fmad=false`` and a host compiler told
+not to contract (its device sums and its host twiddles reproduce AudioLazy's ``dft`` bit for bit).  It includes
+``csrc_common/alz_common.h`` too.  :func:`build_native` builds it after the table.
 """
 from __future__ import annotations
 
@@ -75,6 +80,9 @@ LIBRARIES = {lib.name: lib for lib in (
   Library("stft", "libalz_b200_stft.so", "csrc_stft", "alz_b200_stft.h", ("-fmad=false",), _COMMON),
   Library("resample", "libalz_b200_resample.so", "csrc_resample", "alz_b200_resample.h", ("-fmad=false",), _COMMON),
 )}
+#: the DFT library (``fourier`` binds it)
+DFT = Library("dft", "libalz_b200_dft.so", "csrc_dft", "alz_b200_dft.h",
+              ("-fmad=false", "-Xcompiler", "-ffp-contract=off"), _COMMON)
 #: the filter library (``_capi`` loads it from here unless ``ALZ_B200_LIB`` names another file)
 LIB_PATH = LIBRARIES["filters"].path
 
@@ -93,8 +101,8 @@ def find_nvcc():
 
 
 def build_native(force: bool = False, verbose: bool = False) -> list:
-  """Build every library of :data:`LIBRARIES`; returns their paths."""
-  return [build_library(lib, force=force, verbose=verbose) for lib in LIBRARIES.values()]
+  """Build every library of :data:`LIBRARIES`, then :data:`DFT`; returns their paths."""
+  return [build_library(lib, force=force, verbose=verbose) for lib in list(LIBRARIES.values()) + [DFT]]
 
 
 def build_library(lib: Library, force: bool = False, verbose: bool = False) -> str:
