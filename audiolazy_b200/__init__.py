@@ -11,10 +11,11 @@ batched form ``Zcross`` (flags or per-block counts of many streams); ``lpc_frame
 ``stft`` with their batched forms ``OverlapAdd`` and ``Stft`` (short-time Fourier analysis, resynthesis and
 overlap-add of many streams); ``lagrange`` and ``resample`` with its batched form ``Resampler`` (Lagrange sample-rate
 conversion of many streams); ``dft`` at arbitrary frequencies with its batched form ``Dft`` and the lazy ``dft_frames``
-(the DFT of every frame of many streams).
+(the DFT of every frame of many streams); ``unwrap`` and ``clip`` with their batched forms ``Unwrap`` (phase unwrapping
+of many streams, carried block by block) and ``Clip``.
 
 The per-sample recurrences run in hand-written sm_90a CUDA kernels behind the C ABIs of
-``include/alz_b200.h``, ``include/alz_b200_amdf.h``, ``include/alz_b200_zcross.h``, ``include/alz_b200_lpc.h``, ``include/alz_b200_stft.h``, ``include/alz_b200_resample.h`` and ``include/alz_b200_dft.h``; importing this package does not need a GPU, calling a filter does.
+``include/alz_b200.h``, ``include/alz_b200_amdf.h``, ``include/alz_b200_zcross.h``, ``include/alz_b200_lpc.h``, ``include/alz_b200_stft.h``, ``include/alz_b200_resample.h``, ``include/alz_b200_dft.h`` and ``include/alz_b200_unwrap.h``; importing this package does not need a GPU, calling a filter does.
 """
 from .core import StrategyDict
 from .stream import Stream, StreamTeeHub, thub, tostream, avoid_stream
@@ -33,5 +34,6 @@ from .linear_prediction import (ParCorError, acorr, lag_matrix, toeplitz, levins
 from .spectral import window, wsymm, overlap_add, stft, OverlapAdd, OlaState, Stft, StftState
 from .resampling import lagrange, resample, Resampler, ResampleState
 from .fourier import dft, Dft, DftState, dft_frames
+from .unwrapping import unwrap, Unwrap, UnwrapState, clip, Clip
 
 __version__ = "0.1.0"

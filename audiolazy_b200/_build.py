@@ -24,7 +24,10 @@ The five analysis libraries also include ``csrc_common/alz_common.h``.
 :data:`DFT` is a seventh library, declared next to the table rather than in it: ``libalz_b200_dft.so``, the DFT
 library: ``csrc_dft/*.cu`` behind ``include/alz_b200_dft.h``, compiled with ``-fmad=false`` and a host compiler told
 not to contract (its device sums and its host twiddles reproduce AudioLazy's ``dft`` bit for bit).  It includes
-``csrc_common/alz_common.h`` too.  :func:`build_native` builds it after the table.
+``csrc_common/alz_common.h`` too.  :data:`UNWRAP` is an eighth, declared the same way: ``libalz_b200_unwrap.so``, the
+unwrapping library: ``csrc_unwrap/*.cu`` behind ``include/alz_b200_unwrap.h``, compiled with ``-fmad=false`` (its
+float64 running sums reproduce AudioLazy's ``unwrap`` bit for bit), including ``csrc_common/alz_common.h``.
+:func:`build_native` builds both after the table.
 """
 from __future__ import annotations
 
@@ -83,6 +86,8 @@ LIBRARIES = {lib.name: lib for lib in (
 #: the DFT library (``fourier`` binds it)
 DFT = Library("dft", "libalz_b200_dft.so", "csrc_dft", "alz_b200_dft.h",
               ("-fmad=false", "-Xcompiler", "-ffp-contract=off"), _COMMON)
+#: the unwrap and clip library (``unwrapping`` binds it)
+UNWRAP = Library("unwrap", "libalz_b200_unwrap.so", "csrc_unwrap", "alz_b200_unwrap.h", ("-fmad=false",), _COMMON)
 #: the filter library (``_capi`` loads it from here unless ``ALZ_B200_LIB`` names another file)
 LIB_PATH = LIBRARIES["filters"].path
 
@@ -101,8 +106,8 @@ def find_nvcc():
 
 
 def build_native(force: bool = False, verbose: bool = False) -> list:
-  """Build every library of :data:`LIBRARIES`, then :data:`DFT`; returns their paths."""
-  return [build_library(lib, force=force, verbose=verbose) for lib in list(LIBRARIES.values()) + [DFT]]
+  """Build every library of :data:`LIBRARIES`, then :data:`DFT` and :data:`UNWRAP`; returns their paths."""
+  return [build_library(lib, force=force, verbose=verbose) for lib in list(LIBRARIES.values()) + [DFT, UNWRAP]]
 
 
 def build_library(lib: Library, force: bool = False, verbose: bool = False) -> str:

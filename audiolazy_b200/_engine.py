@@ -46,6 +46,20 @@ def stream_input(x):
   return x, S, T, x.stride(0) if S > 1 else max(T, 1)     # a length-1 axis may carry any stride
 
 
+def stream_input64(x):
+  """As :func:`stream_input`, for calls that also take float64 samples: a CUDA float32 or float64 tensor
+  ``x[streams, samples]`` (1-D: one stream) -> ``(x, S, T, row_stride)``, its rows made contiguous."""
+  torch = torch_mod()
+  if x.dim() == 1:
+    x = x.unsqueeze(0)
+  if x.dtype not in (torch.float32, torch.float64) or x.dim() != 2 or x.device.type != "cuda":
+    raise ValueError("x must be a CUDA float32 or float64 tensor [streams, samples]")
+  if x.stride(1) != 1:
+    x = x.contiguous()
+  S, T = x.shape
+  return x, S, T, x.stride(0) if S > 1 else max(T, 1)
+
+
 def check_state(state, cls, owner, S, device):
   """The checks every streaming state takes before its own: ``state`` is a ``cls`` (from ``<owner>.new_state``) made
   for ``S`` streams on ``device``."""
