@@ -27,7 +27,12 @@ not to contract (its device sums and its host twiddles reproduce AudioLazy's ``d
 ``csrc_common/alz_common.h`` too.  :data:`UNWRAP` is an eighth, declared the same way: ``libalz_b200_unwrap.so``, the
 unwrapping library: ``csrc_unwrap/*.cu`` behind ``include/alz_b200_unwrap.h``, compiled with ``-fmad=false`` (its
 float64 running sums reproduce AudioLazy's ``unwrap`` bit for bit), including ``csrc_common/alz_common.h``.
-:func:`build_native` builds both after the table.
+:data:`PARCOR` is a ninth: ``libalz_b200_parcor.so``, the PARCOR library: ``csrc_parcor/*.cu`` behind
+``include/alz_b200_parcor.h``, compiled with ``-fmad=false`` (its step-down and its restatement of glibc's ``pow``
+reproduce AudioLazy's ``parcor`` bit for bit), including ``csrc_common/alz_common.h``.  It is a library of its own
+rather than a unit of the LPC library, whose kernel set is checked as it stands.
+:func:`build_native` builds :data:`DFT` and :data:`UNWRAP` after the table; ``build()`` builds :data:`PARCOR` after
+them with :func:`build_library`.
 """
 from __future__ import annotations
 
@@ -88,6 +93,8 @@ DFT = Library("dft", "libalz_b200_dft.so", "csrc_dft", "alz_b200_dft.h",
               ("-fmad=false", "-Xcompiler", "-ffp-contract=off"), _COMMON)
 #: the unwrap and clip library (``unwrapping`` binds it)
 UNWRAP = Library("unwrap", "libalz_b200_unwrap.so", "csrc_unwrap", "alz_b200_unwrap.h", ("-fmad=false",), _COMMON)
+#: the PARCOR library (``linear_prediction`` binds it)
+PARCOR = Library("parcor", "libalz_b200_parcor.so", "csrc_parcor", "alz_b200_parcor.h", ("-fmad=false",), _COMMON)
 #: the filter library (``_capi`` loads it from here unless ``ALZ_B200_LIB`` names another file)
 LIB_PATH = LIBRARIES["filters"].path
 

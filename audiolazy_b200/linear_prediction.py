@@ -30,7 +30,7 @@ from .filters import ZFilter
 from .stream import Stream
 
 __all__ = ["ParCorError", "acorr", "lag_matrix", "toeplitz", "levinson_durbin", "lpc", "parcor",
-           "parcor_stable", "lsf", "lsf_stable", "LpcFrames", "LpcState", "lpc_frames"]
+           "parcor_stable", "lsf", "lsf_stable", "LpcFrames", "LpcState", "lpc_frames", "parcor_batch", "ParcorResult"]
 
 
 class ParCorError(ZeroDivisionError):
@@ -202,18 +202,56 @@ def _monic_fir(fir_filt):
   return num
 
 
+def _scaled(terms, c):
+  """``Poly(terms) * c`` of the reference: a zero scalar is the zero polynomial, and zero products are dropped."""
+  if c == 0:
+    return {}
+  return {p: v * c for p, v in terms.items() if v * c != 0}
+
+
 def parcor(fir_filt):
   """Generator of the reflection coefficients of a FIR filter, highest order first (step-down
-  recursion; reference ``lazy_lpc.py:343-395``)."""
-  a = _monic_fir(fir_filt)
-  for m in range(len(a) - 1, 0, -1):
-    k = a[m]
+  recursion; reference ``lazy_lpc.py:343-395``).
+
+  It restates the reference's filter algebra, bit for bit: the polynomial keeps only its nonzero terms, each step is
+  ``(A - k zB) * (1 / (1 - k ** 2))`` (a ZFilter divides by a number through its reciprocal, and ``k ** 2`` is
+  CPython's float pow), so a finite ``k`` whose square overflows raises ``OverflowError``, and a zero ``1 - k ** 2``
+  raises :class:`ParCorError`, both after that ``k`` was yielded.  ``parcor_batch`` evaluates the same on the GPU for
+  many rows whose constant term is 1."""
+  den = fir_filt.denominator
+  if len(den) != 1:
+    raise ValueError("Filter has feedback")
+  num = list(fir_filt.numerator)
+  a = {p: v for p, v in enumerate(num) if v != 0}
+  if den[0] != 1:
+    a = _scaled(a, 1 / den[0])
+  for m in range(len(num) - 1, 0, -1):
+    k = a.get(m, 0.0)
     yield k
+    zb = {m - p: v for p, v in a.items()}                       # fir_filt(1 / z) * z ** -m
+    for p, v in _scaled(zb, k).items():                         # minus k zB
+      s = a[p] + -v if p in a else -v
+      if s != 0:
+        a[p] = s
+      else:
+        a.pop(p, None)
     try:
-      a = [(x - k * y) / (1 - k ** 2) for x, y in zip(a, reversed(a))][:m]
+      r = 1 / (1 - k ** 2)
     except ZeroDivisionError:
       raise ParCorError("Can't find next PARCOR coefficient")
-    a[0] = 1
+    a = _scaled(a, r)
+    c0 = a.get(0, 0)                                            # (fir_filt - fir_filt.numpoly[0]) + 1
+    if c0 != 0:
+      s = a[0] + -c0
+      if s != 0:
+        a[0] = s
+      else:
+        del a[0]
+    s = a[0] + 1 if 0 in a else 1
+    if s != 0:
+      a[0] = s
+    else:
+      a.pop(0, None)
 
 
 def parcor_stable(filt):
@@ -474,3 +512,64 @@ def lpc_frames(seq, order, size, hop=None, window=None, method="kautocor"):
     yield frames(lp.apply(torch.empty((1, 0), dtype=torch.float32, device=device), state=state, final=True))
 
   return Stream(it.chain.from_iterable(pump()))
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Batched PARCOR on the GPU (include/alz_b200_parcor.h)
+# ---------------------------------------------------------------------------------------------------------------------
+
+PARCOR_MAX_LEN = 65
+PARCOR_LIB = _capi.NativeLib(_build.PARCOR.path, "PARCOR", {
+  "alz_parcor_last_error": (ctypes.c_char_p, []),
+  "alz_parcor_f64": (_i32, [_vp, _i64, _i64, _i32, _vp, _vp, _vp, _vp, _vp]),
+}, {_capi.ALZ_ERR_INVALID: ValueError})
+
+ParcorResult = collections.namedtuple("ParcorResult", ["k", "count", "failed", "stable"])
+
+
+def parcor_batch(coef):
+  """The reflection coefficients of many FIR rows at once: for a CUDA float64 tensor ``coef[..., L]`` (any leading
+  shape, ``1 <= L <= 65``, the last dimension contiguous; ``LpcFrames(...).apply(x).coef`` as it comes), a
+  :class:`ParcorResult` of
+
+  * ``k [..., L - 1]`` float64: what ``parcor(ZFilter(row))`` yields, in order (highest order first), NaN past count;
+  * ``count [...]`` int32: how many values it yields;
+  * ``failed [...]`` uint8: 0, 1 where it then raises :class:`ParCorError`, 2 where ``k ** 2`` raises
+    ``OverflowError``, 3 for a row whose constant term is not 1 (not evaluated: NaN k, count 0; :func:`parcor` takes
+    those);
+  * ``stable [...]`` bool: ``parcor_stable(1 / ZFilter(row))``.
+
+  The values equal the reference's bit for bit (a NaN by NaN-ness), ``k ** 2`` included (see
+  ``include/alz_b200_parcor.h``)."""
+  import torch
+  if not isinstance(coef, torch.Tensor):
+    raise TypeError("coef must be a torch tensor, not %s" % type(coef).__name__)
+  if coef.dtype != torch.float64:
+    raise TypeError("coef must be float64 (got %s)" % coef.dtype)
+  if coef.dim() < 1:
+    raise ValueError("coef needs a last dimension of coefficients")
+  L = coef.shape[-1]
+  if not 1 <= L <= PARCOR_MAX_LEN:
+    raise ValueError("rows must have 1 .. %d coefficients (got %d)" % (PARCOR_MAX_LEN, L))
+  if not coef.is_cuda:
+    raise ValueError("coef must be a CUDA tensor")
+  _engine.torch_mod()                                           # a usable CUDA device
+  lead = tuple(coef.shape[:-1])
+  with torch.cuda.device(coef.device):
+    if coef.stride(-1) != 1:
+      coef = coef.contiguous()
+    rows = coef.reshape(-1, L) if coef.numel() else coef.new_empty((0, L))
+    if rows.dim() != 2 or rows.stride(-1) != 1 or (rows.shape[0] > 1 and rows.stride(0) < L):
+      rows = rows.contiguous()
+    n = rows.shape[0]
+    dev = coef.device
+    k = torch.empty((n, L - 1), dtype=torch.float64, device=dev)
+    count = torch.empty((n,), dtype=torch.int32, device=dev)
+    failed = torch.empty((n,), dtype=torch.uint8, device=dev)
+    stable = torch.empty((n,), dtype=torch.uint8, device=dev)
+    if n:
+      PARCOR_LIB.check(PARCOR_LIB.load().alz_parcor_f64(
+        rows.data_ptr(), rows.stride(0), n, L, k.data_ptr(), count.data_ptr(), failed.data_ptr(), stable.data_ptr(),
+        torch.cuda.current_stream(dev).cuda_stream))
+  return ParcorResult(k.reshape(lead + (L - 1,)), count.reshape(lead), failed.reshape(lead),
+                      stable.reshape(lead).bool())
