@@ -13,10 +13,11 @@ overlap-add of many streams); ``lagrange`` and ``resample`` with its batched for
 conversion of many streams); ``dft`` at arbitrary frequencies with its batched form ``Dft`` and the lazy ``dft_frames``
 (the DFT of every frame of many streams); ``unwrap`` and ``clip`` with their batched forms ``Unwrap`` (phase unwrapping
 of many streams, carried block by block) and ``Clip``; ``parcor`` with its batched form ``parcor_batch`` (the
-reflection coefficients and ``parcor_stable`` of many LPC rows, such as ``LpcFrames``' output).
+reflection coefficients and ``parcor_stable`` of many LPC rows, such as ``LpcFrames``' output); ``LpcFilter`` (the
+residual of many streams through their frame-wise LPC analysis filters, and its all-pole resynthesis).
 
 The per-sample recurrences run in hand-written sm_90a CUDA kernels behind the C ABIs of
-``include/alz_b200.h``, ``include/alz_b200_amdf.h``, ``include/alz_b200_zcross.h``, ``include/alz_b200_lpc.h``, ``include/alz_b200_stft.h``, ``include/alz_b200_resample.h``, ``include/alz_b200_dft.h``, ``include/alz_b200_unwrap.h`` and ``include/alz_b200_parcor.h``; importing this package does not need a GPU, calling a filter does.
+``include/alz_b200.h``, ``include/alz_b200_amdf.h``, ``include/alz_b200_zcross.h``, ``include/alz_b200_lpc.h``, ``include/alz_b200_stft.h``, ``include/alz_b200_resample.h``, ``include/alz_b200_dft.h``, ``include/alz_b200_unwrap.h``, ``include/alz_b200_parcor.h`` and ``include/alz_b200_lpcfilt.h``; importing this package does not need a GPU, calling a filter does.
 """
 from .core import StrategyDict
 from .stream import Stream, StreamTeeHub, thub, tostream, avoid_stream
@@ -31,7 +32,8 @@ from .analysis import amdf, AmdfBank, AmdfState
 from .crossing import zcross, Zcross, ZcrossState
 from .io import chunks, WavStream, wav_batch, pcm_to_float32
 from .linear_prediction import (ParCorError, acorr, lag_matrix, toeplitz, levinson_durbin, lpc, parcor, parcor_stable,
-                                lsf, lsf_stable, LpcFrames, LpcState, lpc_frames, parcor_batch, ParcorResult)
+                                lsf, lsf_stable, LpcFrames, LpcState, lpc_frames, parcor_batch, ParcorResult,
+                                LpcFilter, LpcFilterState)
 from .spectral import window, wsymm, overlap_add, stft, OverlapAdd, OlaState, Stft, StftState
 from .resampling import lagrange, resample, Resampler, ResampleState
 from .fourier import dft, Dft, DftState, dft_frames

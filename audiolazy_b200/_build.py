@@ -31,8 +31,12 @@ float64 running sums reproduce AudioLazy's ``unwrap`` bit for bit), including ``
 ``include/alz_b200_parcor.h``, compiled with ``-fmad=false`` (its step-down and its restatement of glibc's ``pow``
 reproduce AudioLazy's ``parcor`` bit for bit), including ``csrc_common/alz_common.h``.  It is a library of its own
 rather than a unit of the LPC library, whose kernel set is checked as it stands.
-:func:`build_native` builds :data:`DFT` and :data:`UNWRAP` after the table; ``build()`` builds :data:`PARCOR` after
-them with :func:`build_library`.
+:data:`LPCFILT` is a tenth: ``libalz_b200_lpcfilt.so``, the LPC filtering library: ``csrc_lpcfilt/*.cu`` behind
+``include/alz_b200_lpcfilt.h``, compiled with ``-fmad=false`` (its analysis and synthesis sums reproduce AudioLazy's
+time-varying ZFilters bit for bit), including ``csrc_common/alz_common.h``.  It too is a library of its own for the
+same reason.
+:func:`build_native` builds :data:`DFT` and :data:`UNWRAP` after the table; ``build()`` builds :data:`PARCOR` and then
+:data:`LPCFILT` after them with :func:`build_library`.
 """
 from __future__ import annotations
 
@@ -95,6 +99,8 @@ DFT = Library("dft", "libalz_b200_dft.so", "csrc_dft", "alz_b200_dft.h",
 UNWRAP = Library("unwrap", "libalz_b200_unwrap.so", "csrc_unwrap", "alz_b200_unwrap.h", ("-fmad=false",), _COMMON)
 #: the PARCOR library (``linear_prediction`` binds it)
 PARCOR = Library("parcor", "libalz_b200_parcor.so", "csrc_parcor", "alz_b200_parcor.h", ("-fmad=false",), _COMMON)
+#: the LPC analysis and synthesis filtering library (``linear_prediction`` binds it)
+LPCFILT = Library("lpcfilt", "libalz_b200_lpcfilt.so", "csrc_lpcfilt", "alz_b200_lpcfilt.h", ("-fmad=false",), _COMMON)
 #: the filter library (``_capi`` loads it from here unless ``ALZ_B200_LIB`` names another file)
 LIB_PATH = LIBRARIES["filters"].path
 

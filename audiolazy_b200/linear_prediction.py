@@ -11,7 +11,9 @@ reference to rounding (tests: 1e-9 relative), not bit for bit.
 Frame-wise analysis runs on the GPU (``include/alz_b200_lpc.h``): :class:`LpcFrames` evaluates
 ``lpc.kautocor`` or ``lpc.kcovar`` of every block of ``Stream(x).blocks(size, hop)`` of many
 streams, continued block by block through an :class:`LpcState`, and :func:`lpc_frames` is its lazy
-form.  Those follow the reference's arithmetic operation for operation (CPython 3.12's compensated
+form.  :class:`LpcFilter` filters many streams with those rows, switched frame by frame: the residual through
+the analysis filters, or an excitation through the all-pole synthesis filters (``include/alz_b200_lpcfilt.h``).
+Those follow the reference's arithmetic operation for operation (CPython 3.12's compensated
 ``sum()`` and, for ``kcovar``, its ZFilter algebra included), so they equal the reference's
 ``lpc.kautocor`` / ``lpc.kcovar`` bit for bit -- not the host strategies of this module, which agree
 with it only to rounding.
@@ -30,7 +32,8 @@ from .filters import ZFilter
 from .stream import Stream
 
 __all__ = ["ParCorError", "acorr", "lag_matrix", "toeplitz", "levinson_durbin", "lpc", "parcor",
-           "parcor_stable", "lsf", "lsf_stable", "LpcFrames", "LpcState", "lpc_frames", "parcor_batch", "ParcorResult"]
+           "parcor_stable", "lsf", "lsf_stable", "LpcFrames", "LpcState", "lpc_frames", "parcor_batch", "ParcorResult",
+           "LpcFilter", "LpcFilterState"]
 
 
 class ParCorError(ZeroDivisionError):
@@ -573,3 +576,128 @@ def parcor_batch(coef):
         torch.cuda.current_stream(dev).cuda_stream))
   return ParcorResult(k.reshape(lead + (L - 1,)), count.reshape(lead), failed.reshape(lead),
                       stable.reshape(lead).bool())
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Frame-wise LPC analysis and synthesis filtering on the GPU (include/alz_b200_lpcfilt.h)
+# ---------------------------------------------------------------------------------------------------------------------
+
+LPCFILT_LIB = _capi.NativeLib(_build.LPCFILT.path, "LPC filter", {
+  "alz_lpcfilt_last_error": (ctypes.c_char_p, []),
+  "alz_lpcfilt_state_bytes": (_i64, [_i64, _i32]),
+  "alz_lpcfilt_state_init": (_i32, [_vp, _i64, _i32, _vp]),
+  "alz_lpcfilt_rows": (_i64, [_i64, _i64, _i64]),
+  "alz_lpcfilt_apply": (_i32, [_vp, _i32, _i64, _vp, _i32, _i64, _vp, _i64, _i64, _i64, _vp, _i64, _i64, _i64, _i32,
+                               _i64, _i32, _vp]),
+}, {_capi.ALZ_ERR_INVALID: ValueError})
+
+LPCFILT_KINDS = {"analysis": 0, "synthesis": 1}
+
+
+def _sample_dtype(torch, dtype, what):
+  if dtype == torch.float32:
+    return 0
+  if dtype == torch.float64:
+    return 1
+  raise ValueError("%s must be torch.float32 or torch.float64" % what)
+
+
+class LpcFilterState(object):
+  """Device state of :class:`LpcFilter` calls over ``n_streams`` streams: the samples consumed (counted here, the
+  same for every stream) and per stream the last ``order`` inputs (analysis) or outputs (synthesis) as float64.  It is
+  made for one (order, hop, kind), stream count and device; a new state is zero, the reference's default ``memory``
+  and ``zero``."""
+
+  def __init__(self, filt, n_streams):
+    torch = _engine.torch_mod()
+    self.n_streams = int(n_streams)
+    if self.n_streams < 0:
+      raise ValueError("n_streams must be >= 0")
+    self.key = filt._key()
+    self.consumed = 0
+    device = torch.device("cuda", torch.cuda.current_device())
+    with torch.cuda.device(device):
+      L = LPCFILT_LIB.load()
+      nbytes = LPCFILT_LIB.check(L.alz_lpcfilt_state_bytes(self.n_streams, filt.order))
+      self.tensor = torch.empty(max(8, nbytes), dtype=torch.uint8, device=device)
+      LPCFILT_LIB.check(L.alz_lpcfilt_state_init(self.tensor.data_ptr(), self.n_streams, filt.order,
+                                                 torch.cuda.current_stream(device).cuda_stream))
+
+  @property
+  def device(self):
+    return self.tensor.device
+
+
+class LpcFilter(object):
+  """Frame-wise LPC filtering of many streams: row ``r`` of a stream's coefficient table (``1, c_1 .. c_order``, as
+  :class:`LpcFrames` gives them) filters that stream's samples ``[r hop, (r + 1) hop)``.  ``kind="analysis"`` is the
+  residual through ``A(z) = 1 + sum(c_k z^-k)``, ``kind="synthesis"`` the all-pole ``1 / A(z)``: the reference's
+  ``1 + sum(held(k) * z ** -k)`` and ``1 / (1 + sum(held(k) * z ** -k))``, ``held(k)`` being each row's ``c_k``
+  repeated ``hop`` times, with their default (zero) memory.
+
+  * ``f.apply(x, coef, state=None)`` -> CUDA tensor ``[S, T]`` of ``dtype`` for a CUDA float32 or float64 ``x[S, T]``
+    and a CUDA float64 ``coef[S, F, order + 1]`` (``LpcFrames(...).apply(x).coef`` as it comes: any strides but along
+    the taps, and a stream stride of 0, from ``expand``, shares one table).  Column 0 is not read.  Row 0 of a call is
+    the row that covers its first sample; ``F`` must be at least ``f.n_rows(state.consumed, T)`` (fewer raise
+    ``ValueError``, where the reference raises when a coefficient Stream ends before its input) and rows past it are
+    not read.  The values are the reference's bit for bit (float64) or their rounding (float32).
+  * ``f.n_rows(consumed, T)`` -> the rows a call on ``T`` samples reads after ``consumed``.
+  * ``f.new_state(S)`` -> :class:`LpcFilterState`, to continue streams block by block; blocks of any lengths give the
+    bits of one call."""
+
+  def __init__(self, order, hop, kind="analysis", dtype=None):
+    self.order = _int_arg("order", order, 0, MAX_ORDER)
+    self.hop = _int_arg("hop", hop, 1, 2 ** 62)
+    if not isinstance(kind, str) or kind not in LPCFILT_KINDS:
+      raise ValueError("kind must be 'analysis' or 'synthesis' (got %r)" % (kind,))
+    self.kind = kind
+    if dtype is None:
+      import torch
+      dtype = torch.float32
+    if str(dtype) not in ("torch.float32", "torch.float64"):
+      raise ValueError("dtype must be torch.float32 or torch.float64")
+    self.dtype = dtype
+
+  def _key(self):
+    return (self.order, self.hop, self.kind)
+
+  def new_state(self, n_streams):
+    return LpcFilterState(self, n_streams)
+
+  def n_rows(self, consumed, T):
+    """Rows a call on ``T`` samples reads after ``consumed`` samples (0 for an empty call)."""
+    consumed = _int_arg("consumed", consumed, 0, 2 ** 62)
+    T = _int_arg("T", T, 0, 2 ** 62)
+    return (consumed + T - 1) // self.hop - consumed // self.hop + 1 if T else 0
+
+  def apply(self, x, coef, state=None):
+    torch = _engine.torch_mod()
+    x, S, T, xs = _engine.stream_input64(x)
+    if not isinstance(coef, torch.Tensor) or coef.dtype != torch.float64 or coef.dim() != 3 or not coef.is_cuda:
+      raise ValueError("coef must be a CUDA float64 tensor [streams, rows, order + 1]")
+    if coef.shape[0] != S or coef.shape[2] != self.order + 1:
+      raise ValueError("coef is %s, x has %d streams and the order is %d: need [%d, rows, %d]"
+                       % (tuple(coef.shape), S, self.order, S, self.order + 1))
+    if coef.device != x.device:
+      raise ValueError("coef lives on %s, x on %s" % (coef.device, x.device))
+    with torch.cuda.device(x.device):
+      if state is None:
+        state = self.new_state(S)
+      _engine.check_state(state, LpcFilterState, "LpcFilter", S, x.device)
+      if state.key != self._key():
+        raise ValueError("state belongs to an LpcFilter with another order, hop or kind")
+      F = coef.shape[1]
+      need = self.n_rows(state.consumed, T)
+      if F < need:
+        raise ValueError("coef has %d rows per stream; %d samples after %d need %d (hop %d)"
+                         % (F, T, state.consumed, need, self.hop))
+      if coef.stride(2) != 1 and self.order > 0:
+        coef = coef.contiguous()
+      out = torch.empty((S, T), dtype=self.dtype, device=x.device)
+      LPCFILT_LIB.check(LPCFILT_LIB.load().alz_lpcfilt_apply(
+        x.data_ptr(), _sample_dtype(torch, x.dtype, "x"), xs, out.data_ptr(),
+        _sample_dtype(torch, self.dtype, "dtype"), max(T, 1), coef.data_ptr(), coef.stride(1) if F > 1 else self.order + 1, coef.stride(0) if S > 1 else 0, F,
+        state.tensor.data_ptr(), S, T, state.consumed, self.order, self.hop, LPCFILT_KINDS[self.kind],
+        torch.cuda.current_stream(x.device).cuda_stream))
+    state.consumed += T
+    return out
