@@ -35,8 +35,11 @@ rather than a unit of the LPC library, whose kernel set is checked as it stands.
 ``include/alz_b200_lpcfilt.h``, compiled with ``-fmad=false`` (its analysis and synthesis sums reproduce AudioLazy's
 time-varying ZFilters bit for bit), including ``csrc_common/alz_common.h``.  It too is a library of its own for the
 same reason.
-:func:`build_native` builds :data:`DFT` and :data:`UNWRAP` after the table; ``build()`` builds :data:`PARCOR` and then
-:data:`LPCFILT` after them with :func:`build_library`.
+:data:`LPCSCAN` is an eleventh: ``libalz_b200_lpcscan.so``, the time-parallel LPC synthesis library:
+``csrc_lpcscan/*.cu`` behind ``include/alz_b200_lpcscan.h``, compiled with ``-fmad=false`` (its walks of a flagged
+stream reproduce the LPC filtering library's synthesis bit for bit), including ``csrc_common/alz_common.h``.
+:func:`build_native` builds :data:`DFT` and :data:`UNWRAP` after the table; ``build()`` builds :data:`PARCOR`,
+:data:`LPCFILT` and then :data:`LPCSCAN` after them with :func:`build_library`.
 """
 from __future__ import annotations
 
@@ -101,6 +104,8 @@ UNWRAP = Library("unwrap", "libalz_b200_unwrap.so", "csrc_unwrap", "alz_b200_unw
 PARCOR = Library("parcor", "libalz_b200_parcor.so", "csrc_parcor", "alz_b200_parcor.h", ("-fmad=false",), _COMMON)
 #: the LPC analysis and synthesis filtering library (``linear_prediction`` binds it)
 LPCFILT = Library("lpcfilt", "libalz_b200_lpcfilt.so", "csrc_lpcfilt", "alz_b200_lpcfilt.h", ("-fmad=false",), _COMMON)
+#: the time-parallel LPC synthesis library (``linear_prediction`` binds it)
+LPCSCAN = Library("lpcscan", "libalz_b200_lpcscan.so", "csrc_lpcscan", "alz_b200_lpcscan.h", ("-fmad=false",), _COMMON)
 #: the filter library (``_capi`` loads it from here unless ``ALZ_B200_LIB`` names another file)
 LIB_PATH = LIBRARIES["filters"].path
 

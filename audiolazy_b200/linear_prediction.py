@@ -12,7 +12,8 @@ Frame-wise analysis runs on the GPU (``include/alz_b200_lpc.h``): :class:`LpcFra
 ``lpc.kautocor`` or ``lpc.kcovar`` of every block of ``Stream(x).blocks(size, hop)`` of many
 streams, continued block by block through an :class:`LpcState`, and :func:`lpc_frames` is its lazy
 form.  :class:`LpcFilter` filters many streams with those rows, switched frame by frame: the residual through
-the analysis filters, or an excitation through the all-pole synthesis filters (``include/alz_b200_lpcfilt.h``).
+the analysis filters, or an excitation through the all-pole synthesis filters (``include/alz_b200_lpcfilt.h``), the
+synthesis of few long streams optionally cut into chunks evaluated in parallel (``include/alz_b200_lpcscan.h``).
 Those follow the reference's arithmetic operation for operation (CPython 3.12's compensated
 ``sum()`` and, for ``kcovar``, its ZFilter algebra included), so they equal the reference's
 ``lpc.kautocor`` / ``lpc.kcovar`` bit for bit -- not the host strategies of this module, which agree
@@ -593,6 +594,14 @@ LPCFILT_LIB = _capi.NativeLib(_build.LPCFILT.path, "LPC filter", {
 
 LPCFILT_KINDS = {"analysis": 0, "synthesis": 1}
 
+LPCSCAN_LIB = _capi.NativeLib(_build.LPCSCAN.path, "time-parallel LPC synthesis", {
+  "alz_lpcscan_last_error": (ctypes.c_char_p, []),
+  "alz_lpcscan_chunks": (_i64, [_i64, _i64, _i32, _i64]),
+  "alz_lpcscan_scratch_bytes": (_i64, [_i64, _i64, _i32]),
+  "alz_lpcscan_apply": (_i32, [_vp, _i32, _i64, _vp, _i32, _i64, _vp, _i64, _i64, _i64, _vp, _i64, _i64, _i64, _i32,
+                               _i64, _i64, _vp, _i64, _vp]),
+}, {_capi.ALZ_ERR_INVALID: ValueError})
+
 
 def _sample_dtype(torch, dtype, what):
   if dtype == torch.float32:
@@ -643,9 +652,20 @@ class LpcFilter(object):
     not read.  The values are the reference's bit for bit (float64) or their rounding (float32).
   * ``f.n_rows(consumed, T)`` -> the rows a call on ``T`` samples reads after ``consumed``.
   * ``f.new_state(S)`` -> :class:`LpcFilterState`, to continue streams block by block; blocks of any lengths give the
-    bits of one call."""
+    bits of one call.
+  * ``f.chunks(S, T)`` -> the chunks per stream a call of that shape is cut into (1: sequential).
 
-  def __init__(self, order, hop, kind="analysis", dtype=None):
+  ``time_parallel`` lets the synthesis of few long streams, which one thread per stream walks slowly, run in chunks
+  (``include/alz_b200_lpcscan.h``): each chunk's response to its start state is summarized, the chunk start states are
+  scanned, and every chunk is rerun from its own.  ``False`` (the default) always walks sequentially; ``True`` lets a
+  cost model pick the chunk count, which is 1 unless the chunks pay; a positive int forces that count, lowered so that
+  every chunk holds at least ``max(order, 1)`` samples.  A call cut into chunks differs from the sequential bits by the
+  float64 rounding drift of the scan (``DESIGN.md`` gives the measured size); a stream whose chunk summaries or scanned
+  states are not finite (NaN or infinite samples or rows, unstable rows that overflow) is walked sequentially in the
+  same launches and keeps its bits.  Calls of either kind mix freely on one state.  The analysis is sample-parallel
+  and exact already, and ignores the option."""
+
+  def __init__(self, order, hop, kind="analysis", dtype=None, time_parallel=False):
     self.order = _int_arg("order", order, 0, MAX_ORDER)
     self.hop = _int_arg("hop", hop, 1, 2 ** 62)
     if not isinstance(kind, str) or kind not in LPCFILT_KINDS:
@@ -657,9 +677,27 @@ class LpcFilter(object):
     if str(dtype) not in ("torch.float32", "torch.float64"):
       raise ValueError("dtype must be torch.float32 or torch.float64")
     self.dtype = dtype
+    if isinstance(time_parallel, bool):
+      self.time_parallel = time_parallel
+    elif isinstance(time_parallel, Integral):
+      if time_parallel < 1:
+        raise ValueError("time_parallel must be True, False or a positive chunk count (got %d)" % time_parallel)
+      self.time_parallel = int(time_parallel)
+    else:
+      raise TypeError("time_parallel must be a bool or a positive int, not %s" % type(time_parallel).__name__)
 
   def _key(self):
     return (self.order, self.hop, self.kind)
+
+  def chunks(self, n_streams, n_samples):
+    """Chunks per stream a call on ``n_streams`` x ``n_samples`` is cut into (1: sequential evaluation)."""
+    S = _int_arg("n_streams", n_streams, 0, 2 ** 62)
+    T = _int_arg("n_samples", n_samples, 0, 2 ** 62)
+    if self.kind != "synthesis" or self.time_parallel is False or self.order == 0:
+      return 1
+    if self.time_parallel is True:
+      return LPCSCAN_LIB.check(LPCSCAN_LIB.load().alz_lpcscan_chunks(S, T, self.order, self.hop))
+    return max(1, min(self.time_parallel, T // self.order))
 
   def new_state(self, n_streams):
     return LpcFilterState(self, n_streams)
@@ -694,10 +732,21 @@ class LpcFilter(object):
       if coef.stride(2) != 1 and self.order > 0:
         coef = coef.contiguous()
       out = torch.empty((S, T), dtype=self.dtype, device=x.device)
-      LPCFILT_LIB.check(LPCFILT_LIB.load().alz_lpcfilt_apply(
-        x.data_ptr(), _sample_dtype(torch, x.dtype, "x"), xs, out.data_ptr(),
-        _sample_dtype(torch, self.dtype, "dtype"), max(T, 1), coef.data_ptr(), coef.stride(1) if F > 1 else self.order + 1, coef.stride(0) if S > 1 else 0, F,
-        state.tensor.data_ptr(), S, T, state.consumed, self.order, self.hop, LPCFILT_KINDS[self.kind],
-        torch.cuda.current_stream(x.device).cuda_stream))
+      P = self.chunks(S, T)
+      stream = torch.cuda.current_stream(x.device).cuda_stream
+      if P > 1:
+        L = LPCSCAN_LIB.load()
+        nbytes = LPCSCAN_LIB.check(L.alz_lpcscan_scratch_bytes(S, P, self.order))
+        # on this stream: torch's allocator orders reuse
+        scratch = torch.empty(max(8, nbytes), dtype=torch.uint8, device=x.device)
+        LPCSCAN_LIB.check(L.alz_lpcscan_apply(
+          x.data_ptr(), _sample_dtype(torch, x.dtype, "x"), xs, out.data_ptr(), _sample_dtype(torch, self.dtype, "dtype"),
+          max(T, 1), coef.data_ptr(), coef.stride(1) if F > 1 else self.order + 1, coef.stride(0) if S > 1 else 0, F,
+          state.tensor.data_ptr(), S, T, state.consumed, self.order, self.hop, P, scratch.data_ptr(), nbytes, stream))
+      else:
+        LPCFILT_LIB.check(LPCFILT_LIB.load().alz_lpcfilt_apply(
+          x.data_ptr(), _sample_dtype(torch, x.dtype, "x"), xs, out.data_ptr(),
+          _sample_dtype(torch, self.dtype, "dtype"), max(T, 1), coef.data_ptr(), coef.stride(1) if F > 1 else self.order + 1, coef.stride(0) if S > 1 else 0, F,
+          state.tensor.data_ptr(), S, T, state.consumed, self.order, self.hop, LPCFILT_KINDS[self.kind], stream))
     state.consumed += T
     return out
