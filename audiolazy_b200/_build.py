@@ -3,43 +3,36 @@
 ``nvcc`` cross-compiles for sm_90a (H100) without a GPU; the built ``.so`` files are git-ignored
 but travel to the GPU box with the repository snapshot.
 
-:data:`LIBRARIES` lists the six libraries.  Each one is the ``.cu`` units of its source directory, compiled in
-parallel into ``_native/obj/<name>/`` (only the units that changed) and linked into one shared library:
+:data:`LIBRARIES` lists the eleven libraries, in build order.  Each one is the ``.cu`` units of its source directory,
+compiled in parallel into ``_native/obj/<name>/`` (only the units that changed) and linked into one shared library.
+Every library but the filter library also includes ``csrc_common/alz_common.h``.  ``-fmad=false`` keeps nvcc from
+fusing a product into an addition, which would round once where AudioLazy rounds twice.
 
-* ``libalz_b200.so``, the filter library: ``csrc/*.cu`` behind ``include/alz_b200.h`` (the C ABI plus one unit of
-  kernel instantiations per cascade length).
-* ``libalz_b200_amdf.so``, the AMDF library: ``csrc_amdf/*.cu`` behind ``include/alz_b200_amdf.h``, compiled with
-  ``-fmad=false`` (its float64 arithmetic reproduces AudioLazy's bit for bit).
-* ``libalz_b200_zcross.so``, the zero-crossing library: ``csrc_zcross/*.cu`` behind ``include/alz_b200_zcross.h``.
-* ``libalz_b200_lpc.so``, the frame-wise LPC library: ``csrc_lpc/*.cu`` behind ``include/alz_b200_lpc.h``, compiled
-  with ``-fmad=false`` (its float64 sums reproduce AudioLazy's bit for bit).
-* ``libalz_b200_stft.so``, the short-time Fourier library: ``csrc_stft/*.cu`` behind ``include/alz_b200_stft.h``,
-  compiled with ``-fmad=false`` (its window products and overlap-add sums reproduce AudioLazy's bit for bit).
-* ``libalz_b200_resample.so``, the Lagrange resampling library: ``csrc_resample/*.cu`` behind
-  ``include/alz_b200_resample.h``, compiled with ``-fmad=false`` (its weights and compensated sums reproduce
-  AudioLazy's bit for bit).
+* ``filters``: ``libalz_b200.so``, ``csrc/*.cu`` behind ``include/alz_b200.h`` (the C ABI plus one unit of kernel
+  instantiations per cascade length).
+* ``amdf``: ``libalz_b200_amdf.so``, ``csrc_amdf/*.cu`` behind ``include/alz_b200_amdf.h``; ``-fmad=false``: its
+  float64 arithmetic reproduces AudioLazy's bit for bit.
+* ``zcross``: ``libalz_b200_zcross.so``, ``csrc_zcross/*.cu`` behind ``include/alz_b200_zcross.h``.
+* ``lpc``: ``libalz_b200_lpc.so``, ``csrc_lpc/*.cu`` behind ``include/alz_b200_lpc.h``; ``-fmad=false``: its float64
+  sums reproduce AudioLazy's bit for bit.
+* ``stft``: ``libalz_b200_stft.so``, ``csrc_stft/*.cu`` behind ``include/alz_b200_stft.h``; ``-fmad=false``: its
+  window products and overlap-add sums reproduce AudioLazy's bit for bit.
+* ``resample``: ``libalz_b200_resample.so``, ``csrc_resample/*.cu`` behind ``include/alz_b200_resample.h``;
+  ``-fmad=false``: its weights and compensated sums reproduce AudioLazy's bit for bit.
+* ``dft``: ``libalz_b200_dft.so``, ``csrc_dft/*.cu`` behind ``include/alz_b200_dft.h``; ``-fmad=false`` and a host
+  compiler told not to contract (``-ffp-contract=off``): its device sums and its host twiddles reproduce AudioLazy's
+  ``dft`` bit for bit.
+* ``unwrap``: ``libalz_b200_unwrap.so``, ``csrc_unwrap/*.cu`` behind ``include/alz_b200_unwrap.h``; ``-fmad=false``:
+  its float64 running sums reproduce AudioLazy's ``unwrap`` bit for bit.
+* ``parcor``: ``libalz_b200_parcor.so``, ``csrc_parcor/*.cu`` behind ``include/alz_b200_parcor.h``; ``-fmad=false``:
+  its step-down and its restatement of glibc's ``pow`` reproduce AudioLazy's ``parcor`` bit for bit.
+* ``lpcfilt``: ``libalz_b200_lpcfilt.so``, ``csrc_lpcfilt/*.cu`` behind ``include/alz_b200_lpcfilt.h``;
+  ``-fmad=false``: its analysis and synthesis sums reproduce AudioLazy's time-varying ZFilters bit for bit.
+* ``lpcscan``: ``libalz_b200_lpcscan.so``, ``csrc_lpcscan/*.cu`` behind ``include/alz_b200_lpcscan.h``;
+  ``-fmad=false``: its walks of a flagged stream reproduce the LPC filtering library's synthesis bit for bit.
 
-The five analysis libraries also include ``csrc_common/alz_common.h``.
-
-:data:`DFT` is a seventh library, declared next to the table rather than in it: ``libalz_b200_dft.so``, the DFT
-library: ``csrc_dft/*.cu`` behind ``include/alz_b200_dft.h``, compiled with ``-fmad=false`` and a host compiler told
-not to contract (its device sums and its host twiddles reproduce AudioLazy's ``dft`` bit for bit).  It includes
-``csrc_common/alz_common.h`` too.  :data:`UNWRAP` is an eighth, declared the same way: ``libalz_b200_unwrap.so``, the
-unwrapping library: ``csrc_unwrap/*.cu`` behind ``include/alz_b200_unwrap.h``, compiled with ``-fmad=false`` (its
-float64 running sums reproduce AudioLazy's ``unwrap`` bit for bit), including ``csrc_common/alz_common.h``.
-:data:`PARCOR` is a ninth: ``libalz_b200_parcor.so``, the PARCOR library: ``csrc_parcor/*.cu`` behind
-``include/alz_b200_parcor.h``, compiled with ``-fmad=false`` (its step-down and its restatement of glibc's ``pow``
-reproduce AudioLazy's ``parcor`` bit for bit), including ``csrc_common/alz_common.h``.  It is a library of its own
-rather than a unit of the LPC library, whose kernel set is checked as it stands.
-:data:`LPCFILT` is a tenth: ``libalz_b200_lpcfilt.so``, the LPC filtering library: ``csrc_lpcfilt/*.cu`` behind
-``include/alz_b200_lpcfilt.h``, compiled with ``-fmad=false`` (its analysis and synthesis sums reproduce AudioLazy's
-time-varying ZFilters bit for bit), including ``csrc_common/alz_common.h``.  It too is a library of its own for the
-same reason.
-:data:`LPCSCAN` is an eleventh: ``libalz_b200_lpcscan.so``, the time-parallel LPC synthesis library:
-``csrc_lpcscan/*.cu`` behind ``include/alz_b200_lpcscan.h``, compiled with ``-fmad=false`` (its walks of a flagged
-stream reproduce the LPC filtering library's synthesis bit for bit), including ``csrc_common/alz_common.h``.
-:func:`build_native` builds :data:`DFT` and :data:`UNWRAP` after the table; ``build()`` builds :data:`PARCOR`,
-:data:`LPCFILT` and then :data:`LPCSCAN` after them with :func:`build_library`.
+PARCOR and LPC filtering are libraries of their own rather than units of the LPC library, because that library's
+kernel set is checked as it stands.
 """
 from __future__ import annotations
 
@@ -94,18 +87,13 @@ LIBRARIES = {lib.name: lib for lib in (
   Library("lpc", "libalz_b200_lpc.so", "csrc_lpc", "alz_b200_lpc.h", ("-fmad=false",), _COMMON),
   Library("stft", "libalz_b200_stft.so", "csrc_stft", "alz_b200_stft.h", ("-fmad=false",), _COMMON),
   Library("resample", "libalz_b200_resample.so", "csrc_resample", "alz_b200_resample.h", ("-fmad=false",), _COMMON),
+  Library("dft", "libalz_b200_dft.so", "csrc_dft", "alz_b200_dft.h",
+          ("-fmad=false", "-Xcompiler", "-ffp-contract=off"), _COMMON),
+  Library("unwrap", "libalz_b200_unwrap.so", "csrc_unwrap", "alz_b200_unwrap.h", ("-fmad=false",), _COMMON),
+  Library("parcor", "libalz_b200_parcor.so", "csrc_parcor", "alz_b200_parcor.h", ("-fmad=false",), _COMMON),
+  Library("lpcfilt", "libalz_b200_lpcfilt.so", "csrc_lpcfilt", "alz_b200_lpcfilt.h", ("-fmad=false",), _COMMON),
+  Library("lpcscan", "libalz_b200_lpcscan.so", "csrc_lpcscan", "alz_b200_lpcscan.h", ("-fmad=false",), _COMMON),
 )}
-#: the DFT library (``fourier`` binds it)
-DFT = Library("dft", "libalz_b200_dft.so", "csrc_dft", "alz_b200_dft.h",
-              ("-fmad=false", "-Xcompiler", "-ffp-contract=off"), _COMMON)
-#: the unwrap and clip library (``unwrapping`` binds it)
-UNWRAP = Library("unwrap", "libalz_b200_unwrap.so", "csrc_unwrap", "alz_b200_unwrap.h", ("-fmad=false",), _COMMON)
-#: the PARCOR library (``linear_prediction`` binds it)
-PARCOR = Library("parcor", "libalz_b200_parcor.so", "csrc_parcor", "alz_b200_parcor.h", ("-fmad=false",), _COMMON)
-#: the LPC analysis and synthesis filtering library (``linear_prediction`` binds it)
-LPCFILT = Library("lpcfilt", "libalz_b200_lpcfilt.so", "csrc_lpcfilt", "alz_b200_lpcfilt.h", ("-fmad=false",), _COMMON)
-#: the time-parallel LPC synthesis library (``linear_prediction`` binds it)
-LPCSCAN = Library("lpcscan", "libalz_b200_lpcscan.so", "csrc_lpcscan", "alz_b200_lpcscan.h", ("-fmad=false",), _COMMON)
 #: the filter library (``_capi`` loads it from here unless ``ALZ_B200_LIB`` names another file)
 LIB_PATH = LIBRARIES["filters"].path
 
@@ -124,8 +112,8 @@ def find_nvcc():
 
 
 def build_native(force: bool = False, verbose: bool = False) -> list:
-  """Build every library of :data:`LIBRARIES`, then :data:`DFT` and :data:`UNWRAP`; returns their paths."""
-  return [build_library(lib, force=force, verbose=verbose) for lib in list(LIBRARIES.values()) + [DFT, UNWRAP]]
+  """Build every library of :data:`LIBRARIES`, in order; returns their paths."""
+  return [build_library(lib, force=force, verbose=verbose) for lib in LIBRARIES.values()]
 
 
 def build_library(lib: Library, force: bool = False, verbose: bool = False) -> str:

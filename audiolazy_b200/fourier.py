@@ -29,7 +29,7 @@ MAX_SIZE = 8192
 MAX_FREQS = 4096
 
 _i32, _i64, _vp = ctypes.c_int32, ctypes.c_int64, ctypes.c_void_p
-LIB = _capi.NativeLib(_build.DFT.path, "DFT", {
+LIB = _capi.NativeLib(_build.LIBRARIES["dft"].path, "DFT", {
   "alz_dft_last_error": (ctypes.c_char_p, []),
   "alz_dft_frames": (_i64, [_i64, _i64, _i32, _i32, _i32]),
   "alz_dft_state_bytes": (_i64, [_i64, _i32]),

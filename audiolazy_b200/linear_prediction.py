@@ -523,7 +523,7 @@ def lpc_frames(seq, order, size, hop=None, window=None, method="kautocor"):
 # ---------------------------------------------------------------------------------------------------------------------
 
 PARCOR_MAX_LEN = 65
-PARCOR_LIB = _capi.NativeLib(_build.PARCOR.path, "PARCOR", {
+PARCOR_LIB = _capi.NativeLib(_build.LIBRARIES["parcor"].path, "PARCOR", {
   "alz_parcor_last_error": (ctypes.c_char_p, []),
   "alz_parcor_f64": (_i32, [_vp, _i64, _i64, _i32, _vp, _vp, _vp, _vp, _vp]),
 }, {_capi.ALZ_ERR_INVALID: ValueError})
@@ -583,7 +583,7 @@ def parcor_batch(coef):
 # Frame-wise LPC analysis and synthesis filtering on the GPU (include/alz_b200_lpcfilt.h)
 # ---------------------------------------------------------------------------------------------------------------------
 
-LPCFILT_LIB = _capi.NativeLib(_build.LPCFILT.path, "LPC filter", {
+LPCFILT_LIB = _capi.NativeLib(_build.LIBRARIES["lpcfilt"].path, "LPC filter", {
   "alz_lpcfilt_last_error": (ctypes.c_char_p, []),
   "alz_lpcfilt_state_bytes": (_i64, [_i64, _i32]),
   "alz_lpcfilt_state_init": (_i32, [_vp, _i64, _i32, _vp]),
@@ -594,7 +594,7 @@ LPCFILT_LIB = _capi.NativeLib(_build.LPCFILT.path, "LPC filter", {
 
 LPCFILT_KINDS = {"analysis": 0, "synthesis": 1}
 
-LPCSCAN_LIB = _capi.NativeLib(_build.LPCSCAN.path, "time-parallel LPC synthesis", {
+LPCSCAN_LIB = _capi.NativeLib(_build.LIBRARIES["lpcscan"].path, "time-parallel LPC synthesis", {
   "alz_lpcscan_last_error": (ctypes.c_char_p, []),
   "alz_lpcscan_chunks": (_i64, [_i64, _i64, _i32, _i64]),
   "alz_lpcscan_scratch_bytes": (_i64, [_i64, _i64, _i32]),

@@ -19,7 +19,7 @@ from .stream import Stream
 __all__ = ["unwrap", "Unwrap", "UnwrapState", "clip", "Clip"]
 
 _i32, _i64, _f64, _vp = ctypes.c_int32, ctypes.c_int64, ctypes.c_double, ctypes.c_void_p
-LIB = _capi.NativeLib(_build.UNWRAP.path, "unwrap", {
+LIB = _capi.NativeLib(_build.LIBRARIES["unwrap"].path, "unwrap", {
   "alz_unwrap_last_error": (ctypes.c_char_p, []),
   "alz_unwrap_state_bytes": (_i64, [_i64]),
   "alz_unwrap_state_init": (_i32, [_vp, _i64, _vp]),

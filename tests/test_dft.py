@@ -1,12 +1,11 @@
 """dft against the reference's goldens on the CPU: the float64 emulation of the header's arithmetic reproduces every
 golden, the library's host twiddles equal cmath.exp(-1j * n * f) bit for bit, the argument and frame-count checks,
-and the checks every native library takes, for the DFT library (_build.DFT)."""
+and the DFT library's SASS."""
 import builtins
 import cmath
 import json
 import os
 import re
-import shutil
 import subprocess
 import sys
 
@@ -14,9 +13,9 @@ import numpy as np
 import pytest
 
 import audiolazy_b200 as ab
-from audiolazy_b200 import _build, _capi, _engine, fourier
-from conftest import GOLDEN, ROOT
-from native_libs import check_exports, check_sm90a, cuobjdump
+from audiolazy_b200 import _build, _engine, fourier
+from conftest import GOLDEN
+from native_libs import cuobjdump
 import dft_emulation as em
 
 sys.path.insert(0, GOLDEN)
@@ -167,49 +166,11 @@ def test_python_argument_errors():
     ab.dft([], [1.])
 
 
-def test_dft_library_exports_exactly_its_header():
-  check_exports(fourier.LIB, _build.DFT.header)
-
-
-def test_dft_library_is_sm90a():
-  check_sm90a(_build.DFT.path)
-
-
-def test_unloadable_dft_library_raises_native_error(tmp_path, monkeypatch):
-  monkeypatch.setattr(fourier.LIB, "cdll", None)
-  monkeypatch.setattr(fourier.LIB, "path", str(tmp_path / "missing.so"))
-  with pytest.raises(_capi.NativeError, match="no CPU fallback"):
-    fourier.LIB.load()
-  junk = tmp_path / "junk.so"
-  junk.write_text("not an ELF file\n")
-  monkeypatch.setattr(fourier.LIB, "path", str(junk))
-  with pytest.raises(_capi.NativeError, match="cannot load"):
-    fourier.LIB.load()
-
-
-def test_dft_staleness_follows_its_sources(tmp_path, monkeypatch):
-  for d in ("include", "audiolazy_b200"):
-    shutil.copytree(os.path.join(ROOT, d), str(tmp_path / d), ignore=shutil.ignore_patterns("_native", "__pycache__"))
-  monkeypatch.setattr(_build, "ROOT", str(tmp_path))
-  lib = _build.DFT
-  os.makedirs(str(tmp_path / _build.NATIVE))
-  open(lib.path, "w").close()
-  for rel, stale in (("audiolazy_b200/csrc_common/alz_common.h", True), ("audiolazy_b200/csrc_dft/alz_dft.cu", True),
-                     ("include/alz_b200_dft.h", True), ("include/alz_b200_lpc.h", False),
-                     ("audiolazy_b200/csrc_stft/alz_stft.cu", False)):
-    for src in lib.units() + lib.headers() + [str(tmp_path / rel)]:
-      os.utime(src, (1000, 1000))
-    os.utime(lib.path, (2000, 2000))
-    assert not _build.is_stale(lib)
-    os.utime(str(tmp_path / rel), (3000, 3000))
-    assert _build.is_stale(lib) == stale, rel
-
-
 def test_dft_library_has_no_fused_multiply_add():
   """Built with -fmad=false: no product is contracted into an add.  The only DFMAs are the Newton steps of the
   library's one correctly rounded division (the normalization's quotient, an out-of-line function), whose IEEE result
   they do not change."""
-  sass = subprocess.run([cuobjdump(), "-sass", _build.DFT.path], capture_output=True, text=True).stdout
+  sass = subprocess.run([cuobjdump(), "-sass", _build.LIBRARIES["dft"].path], capture_output=True, text=True).stdout
   functions = re.split(r"\n\s*Function : ", sass)[1:]
   by_name = {f.split(None, 1)[0]: f for f in functions}
   assert sorted(n for n in by_name if "alz_dft" in n) == sorted(by_name)

@@ -1,10 +1,8 @@
 """LpcFilter on the CPU: the kernels' float64 restatement (tests/lpc_filter_emulation.py) against the reference's own
-outputs (tests/golden/make_lpc_filter.py), the argument and row-count checks, and the checks every native library
-takes, for the LPC filtering library (_build.LPCFILT)."""
+outputs (tests/golden/make_lpc_filter.py), the argument and row-count checks, and the LPC filtering library's SASS."""
 import json
 import os
 import re
-import shutil
 import subprocess
 
 import numpy as np
@@ -14,7 +12,7 @@ import audiolazy_b200 as ab
 from audiolazy_b200 import _build, _capi, linear_prediction as lp
 from conftest import ROOT
 from lpc_filter_emulation import lpc_filter, same_bits
-from native_libs import check_exports, check_sm90a, cuobjdump
+from native_libs import cuobjdump
 
 GOLDEN = np.load(os.path.join(ROOT, "tests", "golden", "lpc_filter_cases.npz"))
 META = json.loads(str(GOLDEN["meta"]))
@@ -140,47 +138,11 @@ def test_library_checks_without_a_device():
 
 # --- the library ----------------------------------------------------------------------------------------------------
 
-def test_lpcfilt_library_exports_exactly_its_header():
-  check_exports(lp.LPCFILT_LIB, _build.LPCFILT.header)
-
-
-def test_lpcfilt_library_is_sm90a():
-  check_sm90a(_build.LPCFILT.path)
-
-
-def test_unloadable_lpcfilt_library_raises_native_error(tmp_path, monkeypatch):
-  monkeypatch.setattr(lp.LPCFILT_LIB, "cdll", None)
-  monkeypatch.setattr(lp.LPCFILT_LIB, "path", str(tmp_path / "missing.so"))
-  with pytest.raises(_capi.NativeError, match="no CPU fallback"):
-    lp.LPCFILT_LIB.load()
-
-
-def test_lpcfilt_is_not_in_the_table():
-  assert "lpcfilt" not in _build.LIBRARIES and _build.LPCFILT.flags == ("-fmad=false",)
-
-
-def test_lpcfilt_staleness_follows_its_sources(tmp_path, monkeypatch):
-  for d in ("include", "audiolazy_b200"):
-    shutil.copytree(os.path.join(ROOT, d), str(tmp_path / d), ignore=shutil.ignore_patterns("_native", "__pycache__"))
-  monkeypatch.setattr(_build, "ROOT", str(tmp_path))
-  lib = _build.LPCFILT
-  os.makedirs(str(tmp_path / _build.NATIVE))
-  open(lib.path, "w").close()
-  for rel, stale in (("audiolazy_b200/csrc_lpcfilt/alz_lpcfilt.cu", True), ("include/alz_b200_lpcfilt.h", True),
-                     ("audiolazy_b200/csrc_common/alz_common.h", True), ("include/alz_b200_lpc.h", False),
-                     ("audiolazy_b200/csrc_parcor/alz_parcor.cu", False)):
-    for src in lib.units() + lib.headers() + [str(tmp_path / rel)]:
-      os.utime(src, (1000, 1000))
-    os.utime(lib.path, (2000, 2000))
-    os.utime(str(tmp_path / rel), (3000, 3000))
-    assert _build.is_stale(lib) == stale, rel
-
-
 def test_lpcfilt_kernels_contract_nothing():
   """Built with -fmad=false: no product is fused into an addition, in any of the 42 kernels (analysis and the
   ring-buffer synthesis for each input and output dtype, the register synthesis for each order 1 .. 32, and the
   analysis state commit for each input dtype)."""
-  sass = subprocess.run([cuobjdump(), "-sass", _build.LPCFILT.path], capture_output=True, text=True).stdout
+  sass = subprocess.run([cuobjdump(), "-sass", _build.LIBRARIES["lpcfilt"].path], capture_output=True, text=True).stdout
   functions = re.split(r"\n\s*Function : ", sass)[1:]
   assert len(functions) == 42
   names = [body.split(None, 1)[0] for body in functions]

@@ -1,11 +1,10 @@
 """Time-parallel LPC synthesis on the CPU: the three passes restated in float64 (tests/lpc_scan_emulation.py) against
 the sequential restatement (tests/lpc_filter_emulation.py) within the bar, on the reference's golden rows and on long
-streams of stable rows; the fallback of streams with non-finite summaries; the cost model; the LpcFilter option; and
-the checks every native library takes, for the time-parallel synthesis library (_build.LPCSCAN)."""
+streams of stable rows; the fallback of streams with non-finite summaries; the cost model; the LpcFilter option; the
+time-parallel synthesis library's argument checks; and its SASS."""
 import json
 import os
 import re
-import shutil
 import subprocess
 
 import numpy as np
@@ -16,7 +15,7 @@ from audiolazy_b200 import _build, _capi, linear_prediction as lp
 from conftest import ROOT
 from lpc_filter_emulation import lpc_filter, same_bits
 from lpc_scan_emulation import chunk_bounds, kautocor_rows, lpc_scan, max_chunks, within_bar
-from native_libs import check_exports, check_sm90a, cuobjdump
+from native_libs import cuobjdump
 
 GOLDEN = np.load(os.path.join(ROOT, "tests", "golden", "lpc_filter_cases.npz"))
 META = json.loads(str(GOLDEN["meta"]))
@@ -202,40 +201,10 @@ def test_apply_needs_a_device():
                                                               torch.zeros((1, 2, 3), dtype=torch.float64))
 
 
-def test_lpcscan_library_exports_exactly_its_header():
-  check_exports(lp.LPCSCAN_LIB, _build.LPCSCAN.header)
-
-
-def test_lpcscan_library_is_sm90a():
-  check_sm90a(_build.LPCSCAN.path)
-
-
-def test_lpcscan_is_not_in_the_table():
-  assert "lpcscan" not in _build.LIBRARIES and _build.LPCSCAN.flags == ("-fmad=false",)
-  assert _build.LPCSCAN.deps == ("csrc_common/alz_common.h",)
-
-
-def test_lpcscan_staleness_follows_its_sources(tmp_path, monkeypatch):
-  for d in ("include", "audiolazy_b200"):
-    shutil.copytree(os.path.join(ROOT, d), str(tmp_path / d), ignore=shutil.ignore_patterns("_native", "__pycache__"))
-  monkeypatch.setattr(_build, "ROOT", str(tmp_path))
-  lib = _build.LPCSCAN
-  os.makedirs(str(tmp_path / _build.NATIVE))
-  open(lib.path, "w").close()
-  for rel, stale in (("audiolazy_b200/csrc_lpcscan/alz_lpcscan.cu", True), ("include/alz_b200_lpcscan.h", True),
-                     ("audiolazy_b200/csrc_common/alz_common.h", True), ("include/alz_b200_lpcfilt.h", False),
-                     ("audiolazy_b200/csrc_lpcfilt/alz_lpcfilt.cu", False)):
-    for src in lib.units() + lib.headers() + [str(tmp_path / rel)]:
-      os.utime(src, (1000, 1000))
-    os.utime(lib.path, (2000, 2000))
-    os.utime(str(tmp_path / rel), (3000, 3000))
-    assert _build.is_stale(lib) == stale, rel
-
-
 def test_lpcscan_walks_contract_nothing():
   """Built with -fmad=false: the 33 walk kernels (the register walk for each order 1 .. 32 and the shared-memory
   walk), which give a flagged stream its sequential bits, hold no DFMA; only the scan contracts."""
-  sass = subprocess.run([cuobjdump(), "-sass", _build.LPCSCAN.path], capture_output=True, text=True).stdout
+  sass = subprocess.run([cuobjdump(), "-sass", _build.LIBRARIES["lpcscan"].path], capture_output=True, text=True).stdout
   functions = re.split(r"\n\s*Function : ", sass)[1:]
   assert len(functions) == 34
   names = [body.split(None, 1)[0] for body in functions]

@@ -213,4 +213,4 @@ for name in sorted({e.name.split("(")[0].strip() for e in prof.events() if e.nam
 
 
 def test_every_lpcscan_kernel_is_launched(torch):
-  check_every_kernel_is_launched(_build.LPCSCAN.path, _LAUNCH_PROBE)
+  check_every_kernel_is_launched(_build.LIBRARIES["lpcscan"].path, _LAUNCH_PROBE)

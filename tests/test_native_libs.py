@@ -1,19 +1,22 @@
 """Every native library of ``_build.LIBRARIES``: it has a Python binding that binds exactly the functions its header
 declares, the library exports them and targets sm_90a, the binding fails loudly when the library cannot be loaded
-(there is no CPU fallback), and the library is rebuilt when a source it depends on changes.  Each library's kernel
-launches are checked next to its GPU tests (``native_libs.check_every_kernel_is_launched``)."""
+(there is no CPU fallback), the libraries are built in the table's order with the flags their bits depend on, and a
+library is rebuilt when a source it depends on changes.  Each library's kernel launches are checked next to its GPU
+tests (``native_libs.check_every_kernel_is_launched``)."""
 import os
 import shutil
 
 import pytest
 
-from audiolazy_b200 import _build, _capi, analysis, crossing, linear_prediction, resampling, spectral
+from audiolazy_b200 import _build, _capi, analysis, crossing, fourier, linear_prediction as lp, resampling, spectral
+from audiolazy_b200 import unwrapping
 from conftest import ROOT
 from native_libs import check_exports, check_sm90a
 
 NAMES = sorted(_build.LIBRARIES)
-BINDINGS = {"filters": _capi.LIB, "amdf": analysis.LIB, "zcross": crossing.LIB, "lpc": linear_prediction.LIB,
-            "stft": spectral.LIB, "resample": resampling.LIB}
+BINDINGS = {"filters": _capi.LIB, "amdf": analysis.LIB, "zcross": crossing.LIB, "lpc": lp.LIB, "stft": spectral.LIB,
+            "resample": resampling.LIB, "dft": fourier.LIB, "unwrap": unwrapping.LIB, "parcor": lp.PARCOR_LIB,
+            "lpcfilt": lp.LPCFILT_LIB, "lpcscan": lp.LPCSCAN_LIB}
 
 
 def test_every_library_has_a_binding():
@@ -46,9 +49,33 @@ def test_unloadable_library_raises_native_error(name, tmp_path, monkeypatch):
     binding.load()
 
 
+def test_build_native_builds_the_table_in_order(monkeypatch):
+  built = []
+  monkeypatch.setattr(_build, "build_library", lambda lib, force=False, verbose=False: built.append(lib.name) or lib.path)
+  assert _build.build_native() == [lib.path for lib in _build.LIBRARIES.values()]
+  assert built == list(_build.LIBRARIES) == ["filters", "amdf", "zcross", "lpc", "stft", "resample", "dft", "unwrap",
+                                             "parcor", "lpcfilt", "lpcscan"]
+
+
+def test_flags_and_dependencies_of_the_bit_exact_libraries():
+  """Every library but the filter library shares csrc_common/alz_common.h and reproduces AudioLazy's bits, so nvcc
+  must not fuse its products into additions (-fmad=false); the DFT library's host twiddles must not be contracted
+  either.  Zero crossings only compare samples: there is nothing to contract."""
+  for name, lib in _build.LIBRARIES.items():
+    if name == "filters":
+      continue
+    assert lib.deps == ("csrc_common/alz_common.h",), name
+    if name == "dft":
+      assert lib.flags == ("-fmad=false", "-Xcompiler", "-ffp-contract=off")
+    elif name == "zcross":
+      assert lib.flags == ()
+    else:
+      assert lib.flags == ("-fmad=false",), name
+
+
 def test_staleness_follows_the_dependencies(tmp_path, monkeypatch):
-  """In a copy of the sources: touching the shared header marks exactly the five analysis libraries stale, touching
-  one library's unit or public header marks only that library stale."""
+  """In a copy of the sources: touching the shared header marks exactly the libraries that include it stale, touching
+  one library's unit, private header or public header marks only that library stale."""
   for d in ("include", "audiolazy_b200"):
     shutil.copytree(os.path.join(ROOT, d), str(tmp_path / d), ignore=shutil.ignore_patterns("_native", "__pycache__"))
   monkeypatch.setattr(_build, "ROOT", str(tmp_path))
@@ -66,10 +93,15 @@ def test_staleness_follows_the_dependencies(tmp_path, monkeypatch):
     os.utime(str(tmp_path / rel), (3000, 3000))
     return sorted(lib.name for lib in libs if _build.is_stale(lib))
 
-  assert stale_after_touching("audiolazy_b200/csrc_common/alz_common.h") == ["amdf", "lpc", "resample", "stft", "zcross"]
+  assert stale_after_touching("audiolazy_b200/csrc_common/alz_common.h") == sorted(set(_build.LIBRARIES) - {"filters"})
   assert stale_after_touching("audiolazy_b200/csrc_lpc/alz_lpc.cu") == ["lpc"]
+  assert stale_after_touching("include/alz_b200_lpc.h") == ["lpc"]
   assert stale_after_touching("include/alz_b200_zcross.h") == ["zcross"]
   assert stale_after_touching("audiolazy_b200/csrc/alz_plan.h") == ["filters"]
   assert stale_after_touching("audiolazy_b200/csrc_stft/alz_stft.cu") == ["stft"]
   assert stale_after_touching("include/alz_b200_stft.h") == ["stft"]
   assert stale_after_touching("audiolazy_b200/csrc_resample/alz_resample.cu") == ["resample"]
+  for name in ("dft", "unwrap", "parcor", "lpcfilt", "lpcscan"):
+    assert stale_after_touching("audiolazy_b200/csrc_%s/alz_%s.cu" % (name, name)) == [name]
+    assert stale_after_touching("include/alz_b200_%s.h" % name) == [name]
+  assert stale_after_touching("audiolazy_b200/csrc_parcor/alz_pow2.h") == ["parcor"]

@@ -1,7 +1,6 @@
 """PARCOR on the CPU: the host ``parcor`` / ``parcor_stable`` and the batched form's restatement against the reference's
 own outputs (tests/golden/make_parcor.py), the restatement of CPython's ``k ** 2`` against the live interpreter, the
-argument checks of ``parcor_batch``, and the checks every native library takes, for the PARCOR library
-(_build.PARCOR)."""
+argument checks of ``parcor_batch`` and of the PARCOR library, and the library's SASS."""
 import ctypes
 import json
 import math
@@ -15,9 +14,9 @@ import numpy as np
 import pytest
 
 import audiolazy_b200 as ab
-from audiolazy_b200 import _build, _capi, linear_prediction as lp
+from audiolazy_b200 import _build, linear_prediction as lp
 from conftest import ROOT
-from native_libs import check_exports, check_sm90a, cuobjdump
+from native_libs import cuobjdump
 from parcor_emulation import parcor_row, same_float
 
 CASES = json.load(open(os.path.join(ROOT, "tests", "golden", "parcor_cases.json")))["cases"]
@@ -176,43 +175,11 @@ def test_library_checks_without_a_device():
     lp.PARCOR_LIB.check(L.alz_parcor_f64(None, 1, 1, 0, None, None, None, None, None))
 
 
-def test_parcor_library_exports_exactly_its_header():
-  check_exports(lp.PARCOR_LIB, _build.PARCOR.header)
-
-
-def test_parcor_library_is_sm90a():
-  check_sm90a(_build.PARCOR.path)
-
-
-def test_unloadable_parcor_library_raises_native_error(tmp_path, monkeypatch):
-  monkeypatch.setattr(lp.PARCOR_LIB, "cdll", None)
-  monkeypatch.setattr(lp.PARCOR_LIB, "path", str(tmp_path / "missing.so"))
-  with pytest.raises(_capi.NativeError, match="no CPU fallback"):
-    lp.PARCOR_LIB.load()
-
-
-def test_parcor_staleness_follows_its_sources(tmp_path, monkeypatch):
-  for d in ("include", "audiolazy_b200"):
-    shutil.copytree(os.path.join(ROOT, d), str(tmp_path / d), ignore=shutil.ignore_patterns("_native", "__pycache__"))
-  monkeypatch.setattr(_build, "ROOT", str(tmp_path))
-  lib = _build.PARCOR
-  os.makedirs(str(tmp_path / _build.NATIVE))
-  open(lib.path, "w").close()
-  for rel, stale in (("audiolazy_b200/csrc_parcor/alz_pow2.h", True), ("audiolazy_b200/csrc_parcor/alz_parcor.cu", True),
-                     ("include/alz_b200_parcor.h", True), ("audiolazy_b200/csrc_common/alz_common.h", True),
-                     ("include/alz_b200_lpc.h", False)):
-    for src in lib.units() + lib.headers() + [str(tmp_path / rel)]:
-      os.utime(src, (1000, 1000))
-    os.utime(lib.path, (2000, 2000))
-    os.utime(str(tmp_path / rel), (3000, 3000))
-    assert _build.is_stale(lib) == stale, rel
-
-
 def test_parcor_kernel_contracts_nothing():
   """Built with -fmad=false: the step-down's products are never contracted into an add.  Each instantiation holds
   the 21 DFMAs alz_pow2.h spells out (the ones glibc's compiled pow executes) and the Newton steps of the correctly
   rounded reciprocal 1 / d, and nothing else fused."""
-  sass = subprocess.run([cuobjdump(), "-sass", _build.PARCOR.path], capture_output=True, text=True).stdout
+  sass = subprocess.run([cuobjdump(), "-sass", _build.LIBRARIES["parcor"].path], capture_output=True, text=True).stdout
   functions = re.split(r"\n\s*Function : ", sass)[1:]
   assert len(functions) == 3
   counts = set()

@@ -200,4 +200,4 @@ for name in sorted({e.name.split("(")[0].strip() for e in prof.events() if e.nam
 
 
 def test_every_parcor_kernel_is_launched(torch):
-  check_every_kernel_is_launched(_build.PARCOR.path, _LAUNCH_PROBE)
+  check_every_kernel_is_launched(_build.LIBRARIES["parcor"].path, _LAUNCH_PROBE)

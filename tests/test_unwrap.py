@@ -1,20 +1,17 @@
 """unwrap and clip without a GPU: the emulation of include/alz_b200_unwrap.h against the reference's answers
 (tests/golden/unwrap_cases.json, made by tests/golden/make_unwrap.py from a reference checkout), the vectorised
-emulation against the plain one, argument errors, and the checks every native library takes, for the unwrap library
-(_build.UNWRAP)."""
+emulation against the plain one, and argument errors."""
 import json
 import math
 import os
-import shutil
 import sys
 
 import numpy as np
 import pytest
 
 import audiolazy_b200 as ab
-from audiolazy_b200 import _build, _capi, unwrapping
-from conftest import GOLDEN, ROOT
-from native_libs import check_exports, check_sm90a
+from audiolazy_b200 import unwrapping
+from conftest import GOLDEN
 import unwrap_emulation as em
 
 sys.path.insert(0, GOLDEN)
@@ -166,49 +163,3 @@ def test_python_argument_errors(golden):
   assert (uw.max_delta, uw.step) == (.5, 3.)
   c = ab.Clip(-0., None)
   assert math.copysign(1, c.low) == -1 and c.high is None
-
-
-def test_unwrap_library_exports_exactly_its_header():
-  check_exports(unwrapping.LIB, _build.UNWRAP.header)
-
-
-def test_unwrap_library_is_sm90a():
-  check_sm90a(_build.UNWRAP.path)
-
-
-def test_unloadable_unwrap_library_raises_native_error(tmp_path, monkeypatch):
-  monkeypatch.setattr(unwrapping.LIB, "cdll", None)
-  monkeypatch.setattr(unwrapping.LIB, "path", str(tmp_path / "missing.so"))
-  with pytest.raises(_capi.NativeError, match="no CPU fallback"):
-    unwrapping.LIB.load()
-  junk = tmp_path / "junk.so"
-  junk.write_text("not an ELF file\n")
-  monkeypatch.setattr(unwrapping.LIB, "path", str(junk))
-  with pytest.raises(_capi.NativeError, match="cannot load"):
-    unwrapping.LIB.load()
-
-
-def test_unwrap_staleness_follows_its_sources(tmp_path, monkeypatch):
-  for d in ("include", "audiolazy_b200"):
-    shutil.copytree(os.path.join(ROOT, d), str(tmp_path / d), ignore=shutil.ignore_patterns("_native", "__pycache__"))
-  monkeypatch.setattr(_build, "ROOT", str(tmp_path))
-  lib = _build.UNWRAP
-  os.makedirs(str(tmp_path / _build.NATIVE))
-  open(lib.path, "w").close()
-  for rel, stale in (("audiolazy_b200/csrc_common/alz_common.h", True),
-                     ("audiolazy_b200/csrc_unwrap/alz_unwrap.cu", True), ("include/alz_b200_unwrap.h", True),
-                     ("include/alz_b200_dft.h", False), ("audiolazy_b200/csrc_dft/alz_dft.cu", False)):
-    for src in lib.units() + lib.headers() + [str(tmp_path / rel)]:
-      os.utime(src, (1000, 1000))
-    os.utime(lib.path, (2000, 2000))
-    assert not _build.is_stale(lib)
-    os.utime(str(tmp_path / rel), (3000, 3000))
-    assert _build.is_stale(lib) == stale, rel
-
-
-def test_build_native_builds_the_unwrap_library_after_the_table(monkeypatch):
-  built = []
-  monkeypatch.setattr(_build, "build_library", lambda lib, force=False, verbose=False: built.append(lib.name) or lib.path)
-  _build.build_native()
-  assert built == list(_build.LIBRARIES) + ["dft", "unwrap"]
-  assert "unwrap" not in _build.LIBRARIES

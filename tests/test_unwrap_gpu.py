@@ -315,4 +315,4 @@ for name in sorted({e.name.split("(")[0].strip() for e in prof.events() if e.nam
 
 
 def test_every_unwrap_kernel_is_launched(torch):
-  check_every_kernel_is_launched(_build.UNWRAP.path, _LAUNCH_PROBE)
+  check_every_kernel_is_launched(_build.LIBRARIES["unwrap"].path, _LAUNCH_PROBE)
