@@ -537,6 +537,10 @@ static int build_biquad(alz_plan* p, const std::vector<std::vector<Sec>>& secs, 
   const int group = env_int("ALZ_TILE_GROUP", 0);
   p->tile_group_forced = group == 1 || group == 2 || group == 4;
   p->tile_group = p->tile_group_forced ? group : (p->fp64_ops <= kTileGroup4MaxFp64 ? 4 : 2);
+  // How groups of 4 tiles leave the SM: warp-wide 512-byte row stores (default), or TMA box stores with ALZ_STORE_PATH=tma
+  // (DESIGN.md section 3: measured on the H100).
+  const char* store_path = getenv("ALZ_STORE_PATH");
+  p->vec_store = !(store_path && !strcmp(store_path, "tma"));
   return ALZ_OK;
 }
 

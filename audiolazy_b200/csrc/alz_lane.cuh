@@ -56,6 +56,8 @@ struct AlzTileArgs {
   // but no prefetch under the compute of the same warp -- for launches that fill the machine);
   // 0 / 1 = one tile at a time with the next one prefetched (latency-bound launches).
   int paired;
+  int vec_store;    // TMA engine, tile groups of 4: a group leaves through 32 warp-wide st.global.v4 (one row's 512 B
+                    // each) instead of TMA box stores (alz_lane_tma.cuh); y, ys and ysS 16-byte aligned
   int C;            // channels of the whole bank (output row index = s*C + c)
   int vec_in;       // 1: x rows are 16-byte aligned (16 B cp.async), 0: 4 B cp.async
   int vec_out;      // 1: y rows are 16-byte aligned (st.v4), 0: scalar stores

@@ -4,8 +4,9 @@
 // samples filtered in place), but the tile is moved by the Tensor Memory Accelerator:
 //   * load : ONE cp.async.bulk.tensor.2d per tile (box 32 samples x 32 streams of x[S][T]),
 //            completion on an mbarrier (complete_tx), issued by lane 0;
-//   * store: ONE cp.async.bulk.tensor.3d per tile (box 32 samples x 1 channel x 32 streams of
-//            y[S][C][T]) straight from the same shared buffer.
+//   * store: ONE cp.async.bulk.tensor.4d per tile (box 32 samples x 1 channel x 32 streams of
+//            y[S][C][T]) straight from the same shared buffer; or, for tile groups of 4 (AlzTileArgs::vec_store),
+//            32 warp-wide st.global.v4 per group, each one row's 512 contiguous bytes.
 // The shared tile is dense [32 rows][128 B] with the hardware 128-byte swizzle (16-byte chunk
 // index XOR row & 7), so the per-lane row accesses (LDS.128 / STS.128, lane = row) are bank
 // conflict free without padding, and ragged edges (S % 32, T % 32) are handled by the TMA's
@@ -78,6 +79,10 @@ __device__ __forceinline__ void alz_bulk_commit() { asm volatile("cp.async.bulk.
 __device__ __forceinline__ void alz_bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;\n" ::: "memory"); }
 __device__ __forceinline__ void alz_bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;\n" ::: "memory"); }
 __device__ __forceinline__ void alz_fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
+__device__ __forceinline__ void alz_st_v4_hint(float* p, float4 v, unsigned long long pol) {
+  asm volatile("st.global.L2::cache_hint.v4.f32 [%0], {%1, %2, %3, %4}, %5;\n"
+               ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w), "l"(pol) : "memory");
+}
 
 // Consumers of a filtered tile.  AlzStoreY (default): the tile goes to y[S][C][T] by TMA.  AlzEnvelopePost: the tile is
 // consumed in place -- rectifier / squarer, float64 one-pole lowpass (reference lazy_analysis.py:440-520: envelope.abs /
@@ -120,7 +125,9 @@ struct AlzEnvelopePost {
   __device__ __forceinline__ void store() { *st = env; }
 };
 
-template <class Core, class Post = AlzStoreY, class CoreArgs>
+// VEC: the vector store path is compiled in, and taken where a.vec_store says so.  Instantiations that never run tile
+// groups of 4 by default leave it out: its code costs the head-FIR instantiations, which spill, more spill traffic.
+template <class Core, class Post = AlzStoreY, bool VEC = false, class CoreArgs>
 __device__ __forceinline__ void alz_run_warp_tma(const AlzTileArgs& a, const CoreArgs& ca, const CUtensorMap* tmx,
                                                  const CUtensorMap* tmy, unsigned char* smem) {
   const int lane = threadIdx.x;
@@ -199,8 +206,10 @@ __device__ __forceinline__ void alz_run_warp_tma(const AlzTileArgs& a, const Cor
   // the output stream (64 x the input bytes for a 64-channel bank) is never read again.  Output tiles are stored
   // evict-first and input tiles loaded evict-last, so the L2 gives up output lines first and a late reader still finds
   // its tile there instead of fetching it from HBM again (DESIGN.md section 3: measured on the H100).
+  const bool vec = VEC && !Post::active && a.vec_store;   // host: tile groups of 4 only
   unsigned long long st_pol = 0, ld_pol = 0;
-  if (lane == 0) { st_pol = alz_l2_evict_first(); ld_pol = alz_l2_evict_last(); }
+  if (lane == 0 || vec) st_pol = alz_l2_evict_first();
+  if (lane == 0) ld_pol = alz_l2_evict_last();
   if (lane == 0 && NG == 1) {   // tile 0 in flight
     alz_mbar_expect_tx(mbar0, ALZ_TMA_TILE_BYTES);
     alz_tma_load_3d(tile0, tmx, tb, ld1, ld2, mbar0, ld_pol);
@@ -219,7 +228,7 @@ __device__ __forceinline__ void alz_run_warp_tma(const AlzTileArgs& a, const Cor
           alz_tma_load_3d(tile0 + (j ^ 1) * ALZ_TMA_TILE_BYTES, tmx, tb + t0 + ALZ_TT, ld1, ld2, mbar0 + 8 * (j ^ 1), ld_pol);
         }
       } else if (j == 0) {
-        if (i > 0) alz_bulk_wait_read0();
+        if (i > 0 && !vec) alz_bulk_wait_read0();   // vector stores: the buffers were read out before the last __syncwarp
         const int n = ntiles - i < NG ? ntiles - i : NG;
         for (int jj = 0; jj < n; ++jj) {
           alz_mbar_expect_tx(mbar0 + 8 * jj, ALZ_TMA_TILE_BYTES);
@@ -235,7 +244,31 @@ __device__ __forceinline__ void alz_run_warp_tma(const AlzTileArgs& a, const Cor
     alz_fence_async_smem();                          // my generic-proxy writes -> visible to the TMA store
     __syncwarp();
     const bool last = i + 1 == ntiles;
-    if (lane == 0 && !(a.exp & 2) && !Post::active) {
+    if (vec) {
+      if (!(a.exp & 2) && (j == NG - 1 || last)) {
+        // The group's tiles 0..j leave row by row: one instruction writes row r's (j + 1) x 128 B, lane l carrying
+        // 16-byte chunk l & 7 of tile l >> 3 (the 128-byte swizzle undone on the read).  A 512-byte piece is four
+        // whole lines of one row, which HBM takes at the rate of a sequential fill (DESIGN.md section 3) where a
+        // TMA box of 32 rows x 128 B does not.  Same clipping as the TMA store: rows past S, samples past the
+        // segment, and the ragged last tile of a row length that is no multiple of 4 (stored after the loop).
+        const int jt = lane >> 3, k = lane & 7;
+        const int ncol = jt < j ? ALZ_TT : (jt == j && !(tail_by_lanes && last) ? nvalid : 0);
+        if (4 * k < ncol) {
+          const long long rows = a.S - s0 < 32 ? a.S - s0 : 32;
+          float* dst = a.y + (a.vP > 0 ? ld2 * a.ysS + (long long)ld1 * a.T : s0 * a.ysS) + (long long)c * a.ys + tb + t0 -
+                       (j - jt) * ALZ_TT + 4 * k;
+          const long long ystr = a.vP > 0 ? a.T : a.ysS;   // virtual streams: the group's rows are consecutive chunks
+          const unsigned char* src = smem + jt * ALZ_TMA_TILE_BYTES;
+#pragma unroll 8
+          for (int rr = 0; rr < rows; ++rr) {
+            alz_st_v4_hint(dst, *reinterpret_cast<const float4*>(src + ((k ^ (rr & 7)) << 4)), st_pol);
+            dst += ystr;
+            src += 128;
+          }
+        }
+        __syncwarp();   // every lane has read the group out: its buffers may be refilled
+      }
+    } else if (lane == 0 && !(a.exp & 2) && !Post::active) {
       if (NG == 1) {
         if (!(tail_by_lanes && last)) alz_tma_store_4d(tmy, tb + t0, st1, st2, st3, tile0 + j * ALZ_TMA_TILE_BYTES, st_pol);   // ragged last tile: stored after the loop
         alz_bulk_commit();
@@ -256,7 +289,7 @@ __device__ __forceinline__ void alz_run_warp_tma(const AlzTileArgs& a, const Cor
     float* dst = a.y + s * a.ysS + (long long)c * a.ys + tbeg + t0;
     for (int j = 0; j < nvalid; ++j) dst[j] = src[(((j >> 2) ^ swz) << 2) | (j & 3)];
   }
-  if (lane == 0) alz_bulk_wait0();                   // all output tiles are globally written before exit
+  if (lane == 0 && !vec) alz_bulk_wait0();           // all output tiles are globally written before exit
   if (valid) core.store(a, r, tlen);
   if constexpr (Post::active) { if (valid) post.store(); }
   if (flag != nullptr && seg + 1 < a.nseg) {         // hand the state to the next segment

@@ -29,6 +29,11 @@ alz_biquad_kernel(const __grid_constant__ AlzTileArgs a, const __grid_constant__
   else alz_run_warp<AlzBiquadCore<K, NB, MONIC, NB0, ZMASK, float>>(a, ca, alz_smem);
 }
 
+// Instantiations with the vector store path of tile groups of 4 (alz_run_warp_tma): all but the head-FIR ones, whose
+// plans (19 FP64 instructions per channel-sample) keep tile group 2 unless ALZ_TILE_GROUP forces 4.
+template <int NB0>
+constexpr bool kVecStore = NB0 != 8;
+
 // TMA variant: same cores, tiles moved by cp.async.bulk.tensor (16-byte aligned rows only).
 template <int K, int NB, int MONIC, int NCOEF, int NB0, int ZMASK>
 __global__ void __launch_bounds__(32, kWarpsPerSmTma)
@@ -36,9 +41,9 @@ alz_biquad_tma_kernel(const __grid_constant__ AlzTileArgs a, const __grid_consta
                       const __grid_constant__ CUtensorMap tmx, const __grid_constant__ CUtensorMap tmy) {
   extern __shared__ __align__(1024) unsigned char alz_smem_tma[];
   if (ca.tier(blockIdx.x) == 0)
-    alz_run_warp_tma<AlzBiquadCore<K, NB, MONIC, NB0, ZMASK, double>>(a, ca, &tmx, &tmy, alz_smem_tma);
+    alz_run_warp_tma<AlzBiquadCore<K, NB, MONIC, NB0, ZMASK, double>, AlzStoreY, kVecStore<NB0>>(a, ca, &tmx, &tmy, alz_smem_tma);
   else
-    alz_run_warp_tma<AlzBiquadCore<K, NB, MONIC, NB0, ZMASK, float>>(a, ca, &tmx, &tmy, alz_smem_tma);
+    alz_run_warp_tma<AlzBiquadCore<K, NB, MONIC, NB0, ZMASK, float>, AlzStoreY, kVecStore<NB0>>(a, ca, &tmx, &tmy, alz_smem_tma);
 }
 
 // Envelope consumer (AlzEnvelopePost): the bank's outputs are rectified / squared, lowpassed and decimated in the kernel;
@@ -113,6 +118,10 @@ static int launch_biquad_chunk(const alz_plan* p, AlzTileArgs ta, const void* bl
     ng = alzi_env_int("ALZ_TMA_PAIRED", ng);     // 0/1 = prefetch pipeline, 2 / 4 = tile groups
     if (ng != 2 && ng != 4) ng = 1;
     ta.paired = ng;
+    // Groups of 4 tiles leave as warp-wide row stores where y allows 16-byte vectors (the TMA map already needs that
+    // of its base and strides; checked here so that the kernel's addressing does not depend on it).
+    ta.vec_store = ng == 4 && kVecStore<NB0> && p->vec_store && ((uintptr_t)ta.y & 15) == 0 && (ta.ys & 3) == 0 && (ta.ysS & 3) == 0 &&
+                   (ta.vP == 0 || (ta.T & 3) == 0);
     ta.exp |= alzi_env_int("ALZ_EXP", 0);
     const size_t smem = ALZ_TMA_SMEM_FOR(ng);
     long long per_sm = 0;
@@ -141,8 +150,9 @@ static int launch_biquad_chunk(const alz_plan* p, AlzTileArgs ta, const void* bl
       }
     }
     if (alzi_env_int("ALZ_LOG_LAUNCH", 0))
-      fprintf(stderr, "alz bank launch: %lld warps, tile group %d, %lld CTAs per SM (%lld slots), %lld segment(s) of %lld samples\n",
-              warps, ng, per_sm, slots, nseg, len);
+      fprintf(stderr, "alz bank launch: %lld warps, tile group %d, %lld CTAs per SM (%lld slots), %lld segment(s) of %lld samples, "
+              "%s stores, %d chunks per stream\n", warps, ng, per_sm, slots, nseg, len, ta.vec_store ? "vector" : "TMA",
+              ta.vP > 0 ? ta.vP : 1);
     if (nseg > 1) {
       const size_t words = (size_t)npos + (size_t)npos * groups;
       unsigned* sync = nullptr;

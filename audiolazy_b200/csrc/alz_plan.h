@@ -57,6 +57,7 @@ struct alz_plan {
   int probe_len = 8192;        // samples per probe signal of the tier decision
   int tile_group = 4;          // TMA engine: tiles moved together by launches that fill the machine (1, 2, 4; alz_capi.cu)
   bool tile_group_forced = false;   // ALZ_TILE_GROUP: tile_group on every TMA launch, whatever its size
+  bool vec_store = true;       // TMA launches of tile group 4 store rows with st.global.v4 (ALZ_STORE_PATH=tma: TMA boxes)
   // TMA bank kernel: CTAs resident per SM with 2 / 4 tile buffers (occupancy query on the plan's first TMA launch; 0 = not
   // yet).  Host threads that race on the first launch store the same value.
   mutable std::atomic<int> tma_ctas_per_sm[2] = {};
