@@ -29,6 +29,8 @@ static int launch_window_t(const alz_plan* p, AlzTileArgs ta, cudaStream_t st) {
     const long long warps = (long long)p->C * groups;
     ta.paired = warps >= (long long)p->sm_count * kWinWarpsPerSm ? 2 : 1;
     ta.groups = (int)groups;
+    if (alzi_env_int("ALZ_LOG_LAUNCH", 0))
+      fprintf(stderr, "alz window launch: %lld warps, paired %d\n", warps, ta.paired);
     void* args[4] = {(void*)&ta, p->win_block, (void*)&tmx, (void*)&tmy};
     ALZ_CUDA(cudaLaunchKernel((const void*)alz_window_tma_kernel<MX, MY, NCOEF>, dim3((unsigned)p->C, (unsigned)groups), dim3(32), args,
                               ALZ_TMA_SMEM_FOR(ta.paired), st));

@@ -386,17 +386,20 @@ class Gpu(object):
     return self.torch.cuda.current_stream().cuda_stream
 
   def run(self, plan, x, xinit=None, yinit=None, splits=None, engine="tma", state_out=False):
-    """``x`` [S][T] through ``plan``; rows padded to a multiple of 4 samples.  engine "tma": 16-byte aligned rows (the
-    TMA engine); "cpasync": the same rows with ALZ_NO_TMA=1; "unaligned": base pointers one float off 16 bytes."""
+    """``x`` [S][T] through ``plan``; rows padded to a multiple of 4 samples, plus 8.  engine "tma": 16-byte aligned
+    rows (the TMA engine); "cpasync": the same rows with ALZ_NO_TMA=1; "unaligned": base pointers one float off 16
+    bytes.  The output buffer starts out as SENTINEL words: every word outside y[S][C][:T] must keep it, and none inside
+    may (the 8 extra samples of each row are where a store past the row's end would land; the stride stays a multiple
+    of 4, so the TMA and vector store paths stay eligible)."""
     torch = self.torch
     x = np.atleast_2d(np.asarray(x, dtype=np.float32))
     S, T = x.shape
     C = plan.n_channels
-    stride = (T + 3) // 4 * 4
+    stride = (T + 3) // 4 * 4 + 8
     off = 1 if engine == "unaligned" else 0
     xb = torch.zeros(S * stride + 4, dtype=torch.float32, device=self.dev)
     xb[off:off + S * stride].view(S, stride)[:, :T] = torch.from_numpy(x).to(self.dev)
-    yb = torch.full((S * C * stride + 4,), float("nan"), dtype=torch.float32, device=self.dev)
+    yb = torch.full((S * C * stride + 4,), SENTINEL, dtype=torch.int32, device=self.dev).view(torch.float32)
     st = torch.empty(max(1, plan.state_doubles(S)), dtype=torch.float64, device=self.dev)
     cur = self.stream()
     plan.state_init(st.data_ptr(), S, xinit, yinit, cur)
@@ -406,8 +409,26 @@ class Gpu(object):
         plan.apply(xb.data_ptr() + 4 * (off + t0), yb.data_ptr() + 4 * (off + t0), st.data_ptr(), S, n, stride, stride, cur)
         t0 += n
       self.torch.cuda.synchronize()
+    check_sentinels(yb, off, (S, C, stride), T)
     y = yb[off:off + S * C * stride].view(S, C, stride)[:, :, :T].cpu().numpy()
     return (y, st.cpu().numpy()) if state_out else y
+
+
+SENTINEL = 0x7FC0DEAD                                 # a NaN no kernel produces
+
+
+def check_sentinels(buf, off, shape, T):
+  """``buf``: the whole float32 output buffer; ``shape`` rows of it from word ``off`` on, of which ``[..., :T]`` were
+  written.  Every other word of the buffer must hold SENTINEL, and no written one may."""
+  import torch
+  w = buf.view(torch.int32)
+  n = int(np.prod(shape))
+  rows = w[off:off + n].view(*shape)
+  outside = torch.cat([w[:off], w[off + n:], rows[..., T:].reshape(-1)])
+  bad = int((outside != SENTINEL).sum())
+  assert bad == 0, "%d words outside the output rows were written" % bad
+  left = int((rows[..., :T] == SENTINEL).sum())
+  assert left == 0, "%d samples of the output rows were never written" % left
 
 
 def _signal(case, S=None, T=None):
@@ -473,22 +494,100 @@ def _plan(gpu, case, **env):
     return gpu.capi.Plan(case.bank, **case.plan_kw)
 
 
-def run_filter_case(gpu, case):
-  """biquad / window / generic: three engines agree bit for bit, block splits are bit-exact, the oracle agrees."""
+#: ALZ_LOG_LAUNCH lines: (tile group, segments, segment length, store path, chunks per stream) of a TMA bank launch;
+#: (warps, tiles moved together) of a TMA window launch
+BANK_LOG = re.compile(r"alz bank launch: \d+ warps, tile group (\d+), .* (\d+) segment\(s\) of (\d+) samples, "
+                      r"(vector|TMA) stores, (\d+) chunks per stream")
+WINDOW_LOG = re.compile(r"alz window launch: (\d+) warps, paired (\d+)")
+
+
+def logged(capfd, fn, pattern=BANK_LOG):
+  """``fn()`` under ALZ_LOG_LAUNCH=1: (its result, the fields of every launch line ``pattern`` matches).  Launches on
+  the cp.async engine log nothing."""
+  capfd.readouterr()
+  with _env(ALZ_LOG_LAUNCH=1):
+    out = fn()
+  fields = [pattern.search(l) for l in capfd.readouterr().err.splitlines()]
+  return out, [tuple(v if v in ("vector", "TMA") else int(v) for v in m.groups()) for m in fields if m]
+
+
+def bits(a):
+  """float32 / float64 array -> its words, for bit-for-bit comparisons (NaN included)."""
+  a = np.ascontiguousarray(a)
+  return a.view(np.int32 if a.dtype == np.float32 else np.int64)
+
+
+#: tile group forced at plan creation (ALZ_TILE_GROUP) and ALZ_STORE_PATH: the launch modes of full-machine launches
+TILE_GROUP_RUNS = [(2, "vec"), (4, "vec"), (4, "tma")]
+
+
+def store_path(plan, group, path):
+  """The store path a TMA bank launch of ``plan`` takes at tile group ``group``: warp-wide vector stores at group 4 on
+  the default path, except in the head-FIR instantiations (NB0 = 8), which leave the vector path out."""
+  return "vector" if group == 4 and path == "vec" and plan.num_taps != 8 else "TMA"
+
+
+def run_tile_groups(gpu, case, x, xg, yg, want, capfd):
+  """The case at tile groups 2 and 4 and on both store paths of group 4, whole and in its block splits: the bits and
+  the final state of the group-1 run ``want``, and every logged launch at the forced group and on its store path."""
+  y1, st1 = want
+  for group, path in TILE_GROUP_RUNS:
+    plan = _plan(gpu, case, ALZ_TILE_GROUP=group, ALZ_STORE_PATH=path)
+    for splits in [None] + ([case.splits] if case.splits else []):
+      what = "%s, tile group %d, %s stores, splits %s" % (case.id, group, path, splits)
+      (y, st), log = logged(capfd, lambda: gpu.run(plan, x, xg, yg, splits=splits, state_out=True))
+      assert log, "%s: no TMA bank launch logged" % what
+      assert all(g == group and p == store_path(plan, group, path) for g, _, _, p, _ in log), (what, log)
+      assert np.array_equal(bits(y), bits(y1)), "%s: output differs from tile group 1" % what
+      assert np.array_equal(bits(st), bits(st1)), "%s: final state differs from tile group 1" % what
+
+
+#: warps per SM of the window kernel (kWinWarpsPerSm): a launch of at least this many warps per SM moves tiles in pairs
+WINDOW_WARPS_PER_SM = 12
+
+
+def run_window_paired(gpu, plan, case, x, xg, yg, want, capfd):
+  """The case's rows tiled up to a launch big enough for paired tiles: every replica row gives the small run's bits
+  and final state."""
+  y1, st1 = want
+  C, d = plan.n_channels, plan.state_doubles_per_recurrence
+  sm = gpu.torch.cuda.get_device_properties(gpu.dev).multi_processor_count
+  S = -(-sm * WINDOW_WARPS_PER_SM // C) * 32 + 5
+  rows = np.arange(S) % case.S
+  (y, st), log = logged(capfd, lambda: gpu.run(plan, x[rows], xg, yg, state_out=True), WINDOW_LOG)
+  assert log and all(p == 2 for _, p in log), "%s: %d streams not paired: %s" % (case.id, S, log)
+  assert np.array_equal(bits(y), bits(y1)[rows]), "%s: paired rows differ from the small run" % case.id
+  assert np.array_equal(bits(st).reshape(d, C, S), bits(st1).reshape(d, C, case.S)[:, :, rows]), \
+    "%s: paired final states differ from the small run" % case.id
+
+
+def run_filter_case(gpu, case, capfd):
+  """biquad / window / generic: three engines agree bit for bit, block splits are bit-exact, the oracle agrees.  The
+  biquad kernels give the same bits at tile groups 2 and 4 on both store paths, the window kernels in paired mode."""
   plan = _plan(gpu, case)
   assert (plan.kind, plan.n_sections, plan.state_doubles_per_recurrence) == \
          (case.expect["kind"], case.expect["n_sections"], case.expect["state"])
   x = _signal(case)
   xo, yo, xg, yg = _seeds(case, plan)
-  y = gpu.run(plan, x, xg, yg)
+  (y, st), log = logged(capfd, lambda: gpu.run(plan, x, xg, yg, state_out=True),
+                        WINDOW_LOG if case.family == "window" else BANK_LOG)
   assert np.array_equal(gpu.run(plan, x, xg, yg, engine="cpasync"), y), "cp.async engine differs from TMA"
   assert np.array_equal(gpu.run(plan, x, xg, yg, engine="unaligned"), y), "unaligned rows differ from TMA"
   if case.splits:
     assert np.array_equal(gpu.run(plan, x, xg, yg, splits=case.splits), y), "block splits are not bit-exact"
+  if case.family == "biquad":
+    assert log and all(l[0] == 1 for l in log), log      # the reference of the tile-group runs: one tile at a time
+    run_tile_groups(gpu, case, x, xg, yg, (y, st), capfd)
+  elif case.family == "window":
+    assert log and all(p == 1 for _, p in log), log
+    run_window_paired(gpu, plan, case, x, xg, yg, (y, st), capfd)
   _check_rows(y, oracle.bank_apply(x, case.bank, xinit=xo, yinit=yo), _row_tol(plan, case), case.id)
 
 
-def run_timepar_case(gpu, case):
+def run_timepar_case(gpu, case, capfd):
+  """Time-parallel against sequential evaluation and the oracle; then at tile group 4 on both store paths, which must
+  give the default run's bits: the chunked launch (virtual streams) on the group's store path, and the T - P L samples
+  left over (1 mod 4: a lane-written ragged tile) in a sequential launch of their own."""
   plan = _plan(gpu, case)
   x = _signal(case)
   before = gpu.capi.launch_count()
@@ -498,9 +597,20 @@ def run_timepar_case(gpu, case):
     slow = gpu.run(plan, x)
   assert rel_err(fast, slow) <= 3e-6
   assert rel_err(fast[:1], oracle.bank_apply(x[:1], case.bank)) <= 1e-5
+  for path in ("vec", "tma"):
+    p4 = _plan(gpu, case, ALZ_TILE_GROUP=4, ALZ_STORE_PATH=path)
+    y, log = logged(capfd, lambda: gpu.run(p4, x))
+    what = "%s, tile group 4, %s stores" % (case.id, path)
+    assert log and all(g == 4 and p == store_path(p4, 4, path) for g, _, _, p, _ in log), (what, log)
+    chunked = [l for l in log if l[4] > 1]
+    assert chunked, (what, log)
+    _, _, L, _, P = chunked[-1]
+    tail = log[-1]
+    assert tail[4] == 1 and tail[2] == case.T - P * L and tail[2] % 4 == case.T % 4 == 1, (what, log)
+    assert np.array_equal(bits(y), bits(fast)), "%s: output differs from the default tile group" % what
 
 
-def run_psum_case(gpu, case):
+def run_psum_case(gpu, case, capfd):
   torch = gpu.torch
   plan = _plan(gpu, case)
   assert plan.kind == KIND_BIQUAD and plan.n_fp32_channels == 0 and plan.monic_mode == 0
@@ -524,7 +634,7 @@ def run_psum_case(gpu, case):
   assert torch.equal(out, out2)
 
 
-def run_envelope_case(gpu, case):
+def run_envelope_case(gpu, case, capfd):
   """The fused envelope consumer in paired mode (64 channels x 1600 streams >= 132 SMs x 24 warps) against the plan's own
   float32 bank output, rectified, lowpassed in float64 and decimated by torch; state carried over two calls."""
   torch = gpu.torch
@@ -567,7 +677,7 @@ def run_envelope_case(gpu, case):
     assert rel_err(outs[0], want) <= 1e-7, decim
 
 
-def run_tilegroup_case(gpu, case):
+def run_tilegroup_case(gpu, case, capfd):
   x = _signal(case)
   ys = []
   for grp in (1, 2, 4):
@@ -580,7 +690,7 @@ def run_tilegroup_case(gpu, case):
   _check_rows(ys[0][rows], oracle.bank_apply(x[rows], case.bank), _row_tol(plan, case), case.id)
 
 
-def run_segment_case(gpu, case):
+def run_segment_case(gpu, case, capfd):
   plan = _plan(gpu, case)
   x = _signal(case)
   y, st = gpu.run(plan, x, state_out=True)
@@ -591,7 +701,7 @@ def run_segment_case(gpu, case):
   _check_rows(y[rows], oracle.bank_apply(x[rows], case.bank), _row_tol(plan, case), case.id)
 
 
-def run_tierorder_case(gpu, case):
+def run_tierorder_case(gpu, case, capfd):
   x = _signal(case)
   ys = []
   for order in (0, 1, 2):
@@ -602,7 +712,7 @@ def run_tierorder_case(gpu, case):
   _check_rows(ys[0], oracle.bank_apply(x, case.bank), _row_tol(plan, case), case.id)
 
 
-def run_wpaired_case(gpu, case):
+def run_wpaired_case(gpu, case, capfd):
   """16 channels x 3200 streams = 1600 warps >= 132 SMs x 12: the window TMA kernel in paired mode."""
   plan = _plan(gpu, case)
   x = _signal(case)
@@ -611,7 +721,7 @@ def run_wpaired_case(gpu, case):
   _check_rows(y[rows], oracle.bank_apply(x[rows], case.bank), _row_tol(plan, case), case.id)
 
 
-def run_misc_case(gpu, case):
+def run_misc_case(gpu, case, capfd):
   """alz_freq_response_f64 against numpy in float64; alz_sum_channels_f32 against a left-to-right float64 sum."""
   torch = gpu.torch
   plan = _plan(gpu, case)
@@ -671,9 +781,9 @@ def launches(gpu):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", CASES, ids=lambda c: c.id)
-def test_kernel_matrix(gpu, launches, case):
+def test_kernel_matrix(gpu, launches, capfd, case):
   _RAN.add(case.id)
-  RUNNERS[case.family](gpu, case)
+  RUNNERS[case.family](gpu, case, capfd)
 
 
 # --------------------------------------------------------------------------------------------------------------------
@@ -700,7 +810,7 @@ def library_kernels():
 
 
 @pytest.mark.gpu
-def test_every_kernel_is_launched(gpu, launches):
+def test_every_kernel_is_launched(gpu, launches, capfd):
   """Runs whatever part of the matrix did not run in this session, then compares the kernels the profiler saw launch
   with the kernels compiled into the library."""
   built = library_kernels()
@@ -708,7 +818,7 @@ def test_every_kernel_is_launched(gpu, launches):
     if case.id not in _RAN:
       _RAN.add(case.id)
       try:
-        RUNNERS[case.family](gpu, case)
+        RUNNERS[case.family](gpu, case, capfd)
       except AssertionError:
         pass                       # reported by test_kernel_matrix; only the launches matter here
   gpu.torch.cuda.synchronize()
